@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Headline benchmark: forward point-clouds / second of the SE(3)-Transformer attention hot path on B200.
+"""Headline benchmark: forward point-clouds / second of the SE(3)-Transformer attention hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg2] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg2] [--impl ours|reference] [--dump-outputs DIR]
 
 Workload = BASELINE.json configs[1] ("cfg2": batch 4, N=1024, dim 512, heads 8, dim_head 64, depth 6, num_degrees 4,
 k-NN 16) per GPU; with N GPUs every rank runs its own batch of 4 clouds (weak scaling, no data-path collective) and the
@@ -9,7 +9,8 @@ returned type-0 features are all-gathered so that every rank holds the whole bat
 
   value  : clouds/s with the inputs already resident in HBM (CUDA events, max over ranks)
   e2e    : clouds/s through the public API with HOST inputs: pinned H2D of feats/coors/mask + forward + D2H of the result
-  roofline: the dominant kernel (fused tcgen05 pairwise kernel): algorithmic FLOPs / CUDA-event time vs measured bf16 peak
+  roofline: the dominant kernel (fused wgmma pairwise kernel): algorithmic FLOPs / CUDA-event time vs the bf16 peak
+  --dump-outputs DIR: after the timed steps, the arrays the last resident step returned, as DIR/<name>.npy (float32)
   cpu_baseline / --impl reference: the numpy oracle (port of the reference algorithm) timed on the host cores on a
            bounded, width-preserving sample, extrapolated by algorithmic FLOPs (the full workload needs ~79 h on CPU).
 """
@@ -90,7 +91,8 @@ def load_peaks():
             p = json.load(f)
         return dict(hbm_gbs=p['hbm_gbs'], bf16_burst=p['bf16_tflops'], bf16_sustained=p.get('bf16_tflops_sustained', p['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    # NVIDIA H100 SXM data sheet (700 W card, dense): a ceiling, not a measured rate
+    return dict(hbm_gbs=3350.0, bf16_burst=989.0, bf16_sustained=989.0, source='H100 SXM data sheet (not measured)')
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -280,6 +282,28 @@ class ClockSampler:
 # ------------------------------------------------------------------------------------------------------------------
 # GPU arm
 # ------------------------------------------------------------------------------------------------------------------
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out, path):
+    """The arrays the timed forward returned in its last step, as float32 .npy files: one per output degree (`type<d>`) or
+    `out` for a single tensor.  An array above its share of DUMP_LIMIT_BYTES is replaced by a fixed, seeded sample of its
+    leading-axis rows (`<name>_rows.npy` holds the row indices), so that two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    items = sorted(out.items()) if isinstance(out, dict) else [('out', out)]
+    share = DUMP_LIMIT_BYTES // max(1, len(items))
+    for key, t in items:
+        name = f'type{key}' if isinstance(out, dict) else key
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > share:
+            per_row = a.nbytes // a.shape[0]
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=max(1, (share - 8 * a.shape[0]) // per_row), replace=False))
+            np.save(os.path.join(path, f'{name}_rows.npy'), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(path, f'{name}.npy'), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def run_ours(args, wl, rank, local_rank, world):
     import torch
     import torch.distributed as dist
@@ -359,7 +383,7 @@ def run_ours(args, wl, rank, local_rank, world):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return ms.item(), res
 
-    for _ in range(max(args.warmup, 3)):
+    for _ in range(args.warmup):
         step_e2e()
     sampler = ClockSampler(local_rank)
     if rank == 0:
@@ -372,12 +396,14 @@ def run_ours(args, wl, rank, local_rank, world):
     ops.PROFILE = []
     if args.profile_range:
         torch.cuda.cudart().cudaProfilerStart()
-    ms_res, _ = timed(lambda: step_resident(dev_inputs), args.steps)
+    ms_res, res_out = timed(lambda: step_resident(dev_inputs), args.steps)
     if args.profile_range:
         torch.cuda.cudart().cudaProfilerStop()
     prof, ops.PROFILE = ops.PROFILE, None
     launches = ops.LAUNCHES - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(res_out, args.dump_outputs)
 
     kern = {}
     detail = {}
@@ -462,7 +488,7 @@ def run_ours(args, wl, rank, local_rank, world):
         torch.cuda.empty_cache()
         parity = sample.gpu_parity(dev)
     line = {
-        'metric': 'point-clouds/sec fwd', 'value': value, 'unit': 'clouds/s', 'n_gpus': world, 'steps': args.steps, 'warmup': max(args.warmup, 3),
+        'metric': 'point-clouds/sec fwd', 'value': value, 'unit': 'clouds/s', 'n_gpus': world, 'steps': args.steps, 'warmup': args.warmup,
         'ms_per_step': ms_res / args.steps, 'higher_is_better': True, 'scaling': 'strong' if args.global_batch else 'weak', 'vs_baseline': None, 'dtype': 'f32',
         'data': 'synthetic',
         'config': {'workload': args.workload, **wl['ctor'], 'batch_per_gpu': b, 'global_batch': b * world, 'n_points': n,
@@ -499,7 +525,8 @@ def main():
     ap.add_argument('--global-batch', type=int, default=0, help='STRONG scaling: fixed global batch split over the ranks (default: weak scaling, the workload batch per rank)')
     ap.add_argument('--radial-scale', type=float, default=1.0, help='weights-sensitivity experiment: scale RadialFunc.net.0.weight (rougher radial functions, higher rank)')
     ap.add_argument('--cuda-graph', action='store_true', help='replay the forward from a CUDA graph (launch-bound small workloads)')
-    ap.add_argument('--profile-range', action='store_true', help='cudaProfilerStart/Stop around the resident timed steps (for ncu --profile-from-start off)')
+    ap.add_argument('--profile-range', action='store_true', help='cudaProfilerStart/Stop around the resident timed steps')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the outputs of the last timed step to DIR/<name>.npy (float32)')
     args = ap.parse_args()
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get('RANK', 0))

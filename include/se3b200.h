@@ -1,4 +1,4 @@
-/* se3b200.h -- C ABI of the B200-native SE(3)-Transformer attention hot path.
+/* se3b200.h -- C ABI of the H100-native SE(3)-Transformer attention hot path.
  *
  * The reference (lucidrains/se3-transformer-pytorch @ e1669ee) has no FFI layer: its boundary is the
  * Python class SE3Transformer.  This header declares the entry points a native replacement of the hot
@@ -38,7 +38,7 @@ extern "C" {
 #define SE3_EINVAL       -1   /* bad argument / unsupported shape */
 #define SE3_ECUDA        -2   /* CUDA runtime error (launch, attribute) */
 #define SE3_RADIAL_MID   128  /* RadialFunc mid_dim, se3_transformer_pytorch.py:278 */
-#define SE3_TILE_E       128  /* edges per tile (UMMA M) */
+#define SE3_TILE_E       128  /* edges per tile (MMA M of one CTA) */
 #define SE3_TILE_O        32  /* output channels per tile */
 #define SE3_TILE_IF        4  /* (in-channel, frequency) pairs per tile step */
 
@@ -79,7 +79,7 @@ int se3_radial_trunk_fwd(const float* feat, int64_t E, int in_dim, int num_pairs
  * the factored form, SURVEY.md A.4).  x: [b,n,Ci,Q], basis_pair: [E,P,Q,F], E = b*n*k.  Edge tiles
  * [tile_begin, tile_begin+tile_count) (128 edges each) are written to T in tile layout
  * [tile_count][ceil(Ci*F/4)][4][ceil(P/4)][128][4] floats (zero padded), so a ConvSE3 can be evaluated in edge chunks
- * (the B200 counterpart of the reference's node-axis `splits`, S:243-252). */
+ * (the counterpart of the reference's node-axis `splits`, S:243-252). */
 int se3_tbuild_fwd(const float* x, const int64_t* idx, const float* basis_pair, int b, int n, int k,
                    int Ci, int P, int Q, int F, int64_t tile_begin, int64_t tile_count, float* T, void* stream);
 
@@ -93,8 +93,8 @@ int se3_pairwise_simt_fwd(const float* g, const float* W3, const float* b3, cons
 int64_t se3_w3_image_bytes(int Co, int Ci, int F);
 int se3_pack_w3(const float* W3, const float* b3, int Co, int Ci, int F, void* image, void* stream);
 
-/* Same contraction as se3_pairwise_simt_fwd on the tcgen05 tensor cores (sm_100a only): g [E,128] fp32 from
- * se3_radial_trunk_fwd (one pair's slice; split to fp16 hi/lo into tensor memory inside the kernel), w_img from
+/* Same contraction as se3_pairwise_simt_fwd on the Hopper tensor cores (wgmma, sm_90a): g [E,128] fp32 from
+ * se3_radial_trunk_fwd (one pair's slice; split to fp16 hi/lo into shared memory inside the kernel), w_img from
  * se3_pack_w3, T from se3_tbuild_fwd. */
 int se3_pairwise_tc_fwd(const float* g, const void* w_img, const float* T,
                         int64_t E, int Co, int Ci, int F, int P, int accumulate, float* out, void* stream);
@@ -135,10 +135,6 @@ int se3_rotate_back_fwd(const float* part0, const float* part1, const float* par
  * global frame, out[e,o,:] = D_lo(e) out'[e,:,o]  (F = 1, Q = P, basis_pair = D_lo). */
 int se3_fold_basis_cm_fwd(const float* S, const float* basis_pair, int64_t E, int Co, int P, int Q, int F, int accumulate,
                           float* out, void* stream);
-
-/* Diagnostic for tools/: as se3_pairwise_lr_fwd; CTA 0 writes clock64 stamps of its warp roles to trace[5][64][8] (u64). */
-int se3_pairwise_lr_trace(const float* U, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F, int P,
-                          int Kp, int accumulate, float* out, unsigned long long* trace, void* stream);
 
 /* ---- production path of distance-only radial functions: low-rank radial basis + edge-aligned frames as one GEMM per
  * (degree_out, |m|) (DESIGN.md 4.5; the same product S:237-254, 326-343 re-associated) ------------------------------------ */
@@ -197,7 +193,7 @@ typedef struct se3_zseg {
  *   mode 2 (|m| > 0):  Z_+ = (f=a: U x'[cplus], f=b: -U x'[cminus]),  Z_- = (f=a: U x'[cminus], f=b: U x'[cplus])   (two planes)
  *   mode 3 (|m| > 0):  the same two planes with three real products per complex one (Gauss): S1 = sum (a+b) c, S2 = sum a (d-c),
  *                      S3 = sum b (c+d), c = x'[cplus], d = x'[cminus]; plane + = S1 - S3, plane - = S1 + S2  (3/4 of mode 2's work)
- * on the tcgen05 tensor cores, Z generated on the fly into tensor memory (3-pass fp16 split, fp32 partial sums drained every
+ * on the Hopper tensor cores, Z generated on the fly into wgmma operand registers (3-pass fp16 split, fp32 partial sums drained every
  * flush_stages (0 = default) stages of 64 K values).  w_img: se3_zgemm_pack of every segment in order.  Co % 128 == 0,
  * (Ci * F) % 4 == 0 (F = 1 for mode 1, else 2; mode 3: Ci % 4 == 0), <= 16 segments (HOST array).  out rows: edge stride out_edge_stride floats, plane c at comp_off{c}. */
 int     se3_zgemm_tile_n(int Co, int mode);

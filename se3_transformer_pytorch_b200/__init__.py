@@ -1,8 +1,8 @@
-"""B200-native SE(3)-Transformer attention hot path -- drop-in for `se3_transformer_pytorch.SE3Transformer`.
+"""H100-native SE(3)-Transformer attention hot path -- drop-in for `se3_transformer_pytorch.SE3Transformer`.
 
     from se3_transformer_pytorch_b200 import SE3Transformer
 
-Same constructor / forward / state_dict as the reference; the hot path runs in hand-written sm_100a CUDA kernels
+Same constructor / forward / state_dict as the reference; the hot path runs in hand-written sm_90a CUDA kernels
 (libse3b200.so, C ABI in include/se3b200.h).  CUDA only, forward only.
 """
 from .model import SE3Transformer, ConvSE3, AttentionSE3, OneHeadedKVAttentionSE3, LinearSE3, NormSE3, Fiber

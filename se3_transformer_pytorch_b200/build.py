@@ -1,7 +1,7 @@
-"""In-tree build of libse3b200.so (hand-written sm_100a kernels + C ABI) with nvcc.
+"""In-tree build of libse3b200.so (hand-written sm_90a kernels + C ABI) with nvcc.
 
 No torch extension machinery: the library exposes a plain C ABI (include/se3b200.h) and is loaded with ctypes.
-nvcc cross-compiles for sm_100a without a GPU, so this runs in the CPU-only dev container too.
+nvcc cross-compiles for sm_90a without a GPU, so the library can be built on a machine without one.
 """
 import hashlib
 import os
@@ -17,7 +17,7 @@ EXTRA_DEFS = os.environ.get('SE3B200_NVCC_DEFS', '').split()
 LIB = os.path.join(PKG, f'libse3b200{TAG}.so')
 STAMP = os.path.join(PKG, f'.libse3b200{TAG}.stamp')
 SOURCES = ['api.cu', 'graph.cu', 'basis.cu', 'radial.cu', 'tbuild.cu', 'pairwise_simt.cu', 'pairwise_tc.cu', 'pairwise_lr.cu', 'zgemm.cu', 'aligned.cu', 'attention.cu', 'elementwise.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '--use_fast_math=false',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '--use_fast_math=false',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-O2']
 
 
@@ -90,7 +90,7 @@ def _build_locked(verbose):
     if failed:
         raise RuntimeError('libse3b200 build failed')
     tmp = f'{LIB}.{os.getpid()}.tmp'
-    subprocess.check_call([nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', tmp, *objs])
+    subprocess.check_call([nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', tmp, *objs])
     os.replace(tmp, LIB)
     with open(STAMP + '.tmp', 'w') as f:
         f.write(_digest())

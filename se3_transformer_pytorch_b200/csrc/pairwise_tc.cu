@@ -5,66 +5,25 @@
 // = RadialFunc.net.6 (se3_transformer_pytorch.py:294,299) + PairwiseConv.forward (S:326-343) + the per-edge
 // mat-vec and sum over degree_in of ConvSE3.forward (S:251-254), in the factored form of SURVEY.md A.4.
 //
-// The only dense contraction, R = g . W3^T  (M = 128 edges, N = 128 (o,i,f) columns, K = 128), runs on the 5th-gen
-// tensor cores (tcgen05.mma, cta_group::1, M128 N128 K16, 16-bit x 16-bit -> fp32 in TMEM).  fp32 parity is kept with a
-// 3-pass fp16 split:  g = g_hi + g_lo, W = W_hi + W_lo with hi = fp16(x), lo = fp16(x - hi): 22 mantissa bits per
-// operand (a bf16 pair carries only 16 and cost 10x the error; mixing bf16 hi with fp16 lo in one MMA is an illegal
-// instruction on sm_100a).  R ~= g_hi W_hi + g_lo W_hi + g_hi W_lo  (24 MMAs per tile).  fp16 range: the host only
-// selects this kernel when |W3| and the LayerNorm-bounded |g| stay below 6e4 (else the fp32 SIMT kernel runs).
-// R never leaves the SM: epilogue warps read the accumulator tile with tcgen05.ld, add the bias and contract it with the
-// per-edge T block (packed fp32x2 FMAs), keeping out[e, 32 o, P] in registers across the whole (i,f) loop.
+// The only dense contraction, R = g . W3^T (M = 128 edges, N = 128 (o,i,f) columns, K = 128), runs on the Hopper tensor
+// cores (wgmma m64n64k16, fp16 x fp16 -> fp32) in the kernel of pairwise_wg.cuh.  fp32 parity is kept with a 3-pass fp16
+// split: g = g_hi + g_lo, W = W_hi + W_lo with hi = fp16(x), lo = fp16(x - hi): 22 mantissa bits per operand.
+// R ~= g_hi W_hi + g_lo W_hi + g_hi W_lo.  fp16 range: the host only selects this kernel when |W3| and the LayerNorm-bounded
+// |g| stay below 6e4 (else the fp32 SIMT kernel runs).  R never leaves the SM: the MMA warpgroups add the bias and contract
+// it with the per-edge T block straight from the accumulator registers.
 //
-// One CTA = (tile of 128 edges) x (block of 32 output channels); it loops over ceil(Ci*F/4) steps.  Per step the
-// column order is n = if_local*32 + o_local.  All operands are pre-imaged in global memory in exactly the layout the
-// kernel wants in shared memory (128-byte-swizzled K-major UMMA tiles; T in [if][p-quad][edge][4]) so every stage is
-// filled by 1-D TMA bulk copies (cp.async.bulk, completion on mbarriers) with no tensor maps.
-//
-// The A operand (the 128 x 128 tile of g, stationary for the whole CTA) lives in TENSOR MEMORY, not shared memory:
-// four epilogue warps read the fp32 rows of g, split them into fp16 hi/lo and tcgen05.st them into 128 TMEM columns;
-// every MMA is the .ts form (A from TMEM, B from smem).  Measured reason: with A in smem each M128 N128 K16 MMA pulls
-// 8 KiB of operands through the 128 B/clk shared-memory port, which (with the TMA writes and the epilogue's LDS)
-// made shared-memory bandwidth, not the tensor pipe, the limiter (profiles/r01_*).
-//
-// Warp roles (384 threads): warp 0 = W producer, warp 1 = TMEM owner + MMA issuer, warp 2 = T/bias producer (warp 3 idle; the warpgroup
-// gives its registers away with setmaxnreg), warps 4-11 = epilogue (two warps per TMEM lane quarter, each taking
-// 16 of the 32 output channels, 208 registers each).
-// Pipelines: a ring of five 32 KiB W slots, one per (step, k-half) unit (warp 0 -> MMA, released by tcgen05.commit),
-// a ring of 3-4 T/bias stages (warp 2 -> epilogue; its own producer so T prefetch is not throttled by the W ring),
-// TMEM accumulator double buffer (MMA -> epilogue).
-// Thread-block clusters of CSZ CTAs (same channel block, CSZ consecutive edge tiles) share every W unit: each CTA
-// fetches 1/CSZ of it and multicasts it into all members' shared memory (cp.async.bulk ... .multicast::cluster), and
-// a W slot is recycled when every member's MMAs have retired (tcgen05.commit ... .multicast::cluster).  This cuts the
-// per-SM L2 ingest (the measured limiter: ~80 KiB per 1536-cycle step without it) by the W share.
-// Clusters are rasterised in bands (band_m tile groups x all channel blocks, band_o channel blocks at a time) so that
-// the CTAs resident together share T tiles and W tiles through L2.
+// All operands are pre-imaged in global memory in exactly the layout the kernel wants in shared memory (128-byte-swizzled
+// K-major tiles; T in [if][p-quad][edge][4]) so every stage is filled by 1-D TMA bulk copies (cp.async.bulk, completion on
+// mbarriers) with no tensor maps.
 #include "common.cuh"
-#include "tc_ptx.cuh"
-#include <cuda_bf16.h>
+#include "pairwise_wg.cuh"
 #include <cuda_fp16.h>
-#include <cstdlib>
-#include <algorithm>
 
 namespace se3 {
 
-constexpr int kTcThreads = 384;                // warpgroup 0: TMA + MMA (+2 idle warps); warpgroups 1,2: epilogue
-constexpr uint32_t kImgBytes = 65536;            // one 128x128 hi+lo operand image (4 sub-tiles of 16 KiB)
-constexpr uint32_t kBiasBytes = 512;             // 128 fp32
-constexpr uint32_t kWTileBytes = kImgBytes + kBiasBytes;
-constexpr uint32_t kTmemCols = 512;              // 2 accumulator buffers x 128 columns + A hi/lo (64 + 64 columns)
-constexpr uint32_t kTmemAHi = 256, kTmemALo = 320;
-constexpr uint32_t kUnitBytes = 32768;           // one k-half of a W tile: [hi 16 KiB | lo 16 KiB]
-#ifndef SE3_W_SLOTS
-#define SE3_W_SLOTS 5
-#endif
-#ifndef SE3_T_STAGES_P1
-#define SE3_T_STAGES_P1 4
-#endif
-#ifndef SE3_T_STAGES_P2
-#define SE3_T_STAGES_P2 3
-#endif
-constexpr int kWSlots = SE3_W_SLOTS;
-template <int PH> struct TStages { static constexpr int value = (PH == 1) ? SE3_T_STAGES_P1 : SE3_T_STAGES_P2; };   // T / bias ring depth (smem budget)
-
+constexpr uint32_t kImgBytes = 2 * kPwUnitBytes;  // one 128x128 hi+lo operand image (4 sub-tiles of 16 KiB)
+constexpr uint32_t kWTileBytes = kImgBytes + kPwBiasBytes;
+constexpr uint32_t kUnitBytes = kPwUnitBytes;     // one k-half of a W tile: [hi 16 KiB | lo 16 KiB]
 
 // ---------------------------------------------------------------------------------------------------------
 // weight image packer: W3 fp32 [Co*Ci*F, 128] -> per (o-block, if-block) tile: [hi k0|lo k0|hi k1|lo k1|bias fp32 x128]
@@ -88,393 +47,37 @@ __global__ void pack_w3_kernel(const float* __restrict__ W3, const float* __rest
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------
-// the fused kernel
-// ---------------------------------------------------------------------------------------------------------
-struct TcSmem {                                   // offsets from the 1024-aligned base
-  static constexpr uint32_t W0 = 0;
-  static constexpr uint32_t T0 = kWSlots * kUnitBytes;
-};
-
-struct TcParams {
-  const float* g;
-  const uint8_t* w_img;
-  const float* T;
-  float* out;
-  float* dumpR;
-  int64_t E;
-  int Co, NIFB, n_mt, n_ob, accumulate, dbg, band_m, band_o;
-};
-
-template <int P, int CSZ, bool kDumpR>
-__global__ void __launch_bounds__(kTcThreads, 1)
-pairwise_tc_kernel(const TcParams prm) {
-  const float* __restrict__ g = prm.g;
-  const uint8_t* __restrict__ w_img = prm.w_img;
-  const float* __restrict__ T = prm.T;
-  float* __restrict__ out = prm.out;
-  float* __restrict__ dumpR = prm.dumpR;
-  const int64_t E = prm.E;
-  const int Co = prm.Co, NIFB = prm.NIFB, n_mt = prm.n_mt, n_ob = prm.n_ob, accumulate = prm.accumulate, dbg = prm.dbg;
-  constexpr int PH = (P + 3) / 4;
-  constexpr uint32_t kTBytes = PH * 8192u;         // 4 (i,f) x PH x 128 edges x 16 B
-  constexpr int kTStages = TStages<PH>::value;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - raw);
-  const uint32_t sW = base + TcSmem::W0;           // + slot * kUnitBytes
-  const uint32_t sT = base + TcSmem::T0;           // + st * kTBytes
-  const uint32_t sBias = sT + kTStages * kTBytes;  // + stage * kBiasBytes
-  const uint32_t sBar = sBias + kTStages * kBiasBytes;   // 8-byte barriers
-  // barrier ids
-  const uint32_t bar_a_full = sBar + 0;
-  const uint32_t bar_w_full = sBar + 8;                       // [kWSlots]
-  const uint32_t bar_w_empty = bar_w_full + 8 * kWSlots;      // [kWSlots]
-  const uint32_t bar_t_full = bar_w_empty + 8 * kWSlots;      // [kTStages]
-  const uint32_t bar_t_empty = bar_t_full + 8 * kTStages;     // [kTStages]
-  const uint32_t bar_tm_full = bar_t_empty + 8 * kTStages;    // [2]
-  const uint32_t bar_tm_empty = bar_tm_full + 16;             // [2]
-  const uint32_t s_tmem_slot = bar_tm_empty + 16;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + (s_tmem_slot - base));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // band rasterisation of the 1-D grid of clusters -> (edge-tile group, channel block); rank inside the cluster -> edge tile
-  const uint32_t crank = (CSZ > 1) ? cluster_ctarank() : 0u;
-  constexpr uint16_t kMask = (uint16_t)((1u << CSZ) - 1u);
-  int64_t mt;
-  int ob;
-  bool active;
-  {
-    const int64_t cid = blockIdx.x / CSZ;
-    const int n_mg = (n_mt + CSZ - 1) / CSZ;
-    const int64_t per_band = (int64_t)prm.band_m * n_ob;
-    const int64_t band = cid / per_band;
-    const int64_t r = cid - band * per_band;
-    const int64_t g0 = band * prm.band_m;
-    const int rows = (int)min((int64_t)prm.band_m, (int64_t)n_mg - g0);
-    const int go = (n_ob % prm.band_o == 0) ? prm.band_o : 1;
-    const int64_t chunk = r / ((int64_t)rows * go);
-    const int64_t rr = r - chunk * rows * go;
-    ob = (int)(chunk * go + rr % go);
-    mt = (g0 + rr / go) * CSZ + crank;
-    active = mt < n_mt;
-    if (!active) mt = n_mt - 1;               // padding CTA of the last cluster: same traffic pattern, no stores
-  }
-  if (threadIdx.x == 0) {
-    mbar_init(bar_a_full, 4);                   // one arrival per A-filling warp
-    for (int s = 0; s < kWSlots; ++s) {
-      mbar_init(bar_w_full + 8 * s, 1);
-      mbar_init(bar_w_empty + 8 * s, CSZ);     // one tcgen05.commit arrival from every CTA of the cluster
-    }
-    for (int s = 0; s < kTStages; ++s) {
-      mbar_init(bar_t_full + 8 * s, 1);
-      mbar_init(bar_t_empty + 8 * s, 8);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_tm_full + 8 * s, 1);
-      mbar_init(bar_tm_empty + 8 * s, 8);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_tmem_slot), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (CSZ > 1) cluster_sync_all();            // peers' barriers are initialised before any multicast / remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      const uint8_t* wsrc = w_img + (size_t)ob * NIFB * kWTileBytes;
-      for (int s = 0; s < NIFB; ++s) {
-#pragma unroll
-        for (int kh = 0; kh < 2; ++kh) {
-          const int u = 2 * s + kh;
-          const int slot = u % kWSlots;
-          const uint32_t wph = (uint32_t)(u / kWSlots) & 1u;
-          mbar_wait(bar_w_empty + 8 * slot, wph ^ 1u);
-          mbar_arrive_expect_tx(bar_w_full + 8 * slot, kUnitBytes);
-          if (CSZ == 1) {
-            bulk_g2s(sW + slot * kUnitBytes, wsrc + (size_t)s * kWTileBytes + kh * kUnitBytes, kUnitBytes, bar_w_full + 8 * slot);
-          } else {
-            constexpr uint32_t kShare = kUnitBytes / CSZ;      // this CTA's slice, multicast into every member's slot
-            bulk_g2s_mc(sW + slot * kUnitBytes + crank * kShare, wsrc + (size_t)s * kWTileBytes + kh * kUnitBytes + crank * kShare,
-                        kShare, bar_w_full + 8 * slot, kMask);
-          }
-        }
-      }
-    }
-  } else if (warp == 2) {
-    // ===================== T / bias producer =====================
-    if (lane == 0) {
-      const uint8_t* wsrc = w_img + (size_t)ob * NIFB * kWTileBytes;
-      const uint8_t* tsrc = reinterpret_cast<const uint8_t*>(T) + (size_t)mt * NIFB * kTBytes;
-      for (int s = 0; s < NIFB; ++s) {
-        const int ts = s % kTStages;
-        const uint32_t tph = (uint32_t)(s / kTStages) & 1u;
-        mbar_wait(bar_t_empty + 8 * ts, tph ^ 1u);
-        mbar_arrive_expect_tx(bar_t_full + 8 * ts, kTBytes + kBiasBytes);
-        bulk_g2s(sT + ts * kTBytes, tsrc + (size_t)s * kTBytes, kTBytes, bar_t_full + 8 * ts);
-        bulk_g2s(sBias + ts * kBiasBytes, wsrc + (size_t)s * kWTileBytes + kImgBytes, kBiasBytes, bar_t_full + 8 * ts);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      mbar_wait(bar_a_full, 0);
-      tc_fence_after();
-      for (int s = 0; s < NIFB; ++s) {
-        const int st = s & 1;
-        const uint32_t ph = (uint32_t)(s >> 1) & 1u;
-        mbar_wait(bar_tm_empty + 8 * st, ph ^ 1u);
-        const uint32_t d_tmem = tmem_base + (uint32_t)st * 128u;
-        uint32_t accum = 0;
-#pragma unroll
-        for (int kh = 0; kh < 2; ++kh) {
-          const int u = 2 * s + kh;
-          const int slot = u % kWSlots;
-          const uint32_t wph = (uint32_t)(u / kWSlots) & 1u;
-          mbar_wait(bar_w_full + 8 * slot, wph);
-          tc_fence_after();
-          const uint32_t wbase = sW + slot * kUnitBytes;
-          // pass 0: g_hi x W_hi   pass 1: g_lo x W_hi   pass 2: g_hi x W_lo   (this k-half)
-#pragma unroll
-          for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t a_tmem = tmem_base + ((pass == 1) ? kTmemALo : kTmemAHi) + (uint32_t)(kh * 32);   // 32 columns = 64 k
-            const uint32_t b_part = (pass == 2) ? kSubBytes : 0u;
-#pragma unroll
-            for (int k16 = 0; k16 < 4; ++k16) {
-              const uint64_t bd = umma_desc_sw128(wbase + b_part + k16 * 32);
-              if (!(dbg & 2)) tc_mma_f16_ts(d_tmem, a_tmem + (uint32_t)(k16 * 8), bd, kIdescF16, accum);
-              accum = 1;
-            }
-          }
-          if (CSZ == 1) tc_commit(bar_w_empty + 8 * slot);    // W slot free once these MMAs retire ...
-          else tc_commit_mc(bar_w_empty + 8 * slot, kMask);   // ... in every CTA of the cluster
-        }
-        tc_commit(bar_tm_full + 8 * st);        // accumulator ready for the epilogue
-      }
-    }
-  }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    // ===================== epilogue warps =====================
-    const int q = warp & 3;                    // TMEM lane quarter this warp may access
-    const int half = (warp - 4) >> 2;          // which 16 of the 32 output channels
-    const int el = q * 32 + lane;              // edge row inside the tile
-    const uint32_t t_lane = ((uint32_t)(q * 32)) << 16;
-    if (half == 0) {
-      // ---- A operand: this thread's edge row of g (fp32) -> fp16 hi / lo pairs -> tensor memory
-      const int64_t eg = mt * SE3_TILE_E + el;
-      const float4* grow = reinterpret_cast<const float4*>(g + (size_t)(eg < E ? eg : 0) * SE3_RADIAL_MID);
-      const bool live = eg < E;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {              // 32 k values -> 16 packed columns per chunk
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int v = 0; v < 8; ++v) {
-          float4 x = live ? grow[c * 8 + v] : make_float4(0.f, 0.f, 0.f, 0.f);
-          const float xs[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {
-            const __half h0 = __float2half_rn(xs[2 * h2]), h1 = __float2half_rn(xs[2 * h2 + 1]);
-            const __half l0 = __float2half_rn(xs[2 * h2] - __half2float(h0));
-            const __half l1 = __float2half_rn(xs[2 * h2 + 1] - __half2float(h1));
-            hi[v * 2 + h2] = (uint32_t)__half_as_ushort(h0) | ((uint32_t)__half_as_ushort(h1) << 16);
-            lo[v * 2 + h2] = (uint32_t)__half_as_ushort(l0) | ((uint32_t)__half_as_ushort(l1) << 16);
-          }
-        }
-        tmem_st16(tmem_base + t_lane + kTmemAHi + (uint32_t)(c * 16), hi);
-        tmem_st16(tmem_base + t_lane + kTmemALo + (uint32_t)(c * 16), lo);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_a_full);
-    }
-    unsigned long long acc[8][P];
-#pragma unroll
-    for (int a = 0; a < 8; ++a)
-#pragma unroll
-      for (int p = 0; p < P; ++p) acc[a][p] = 0ull;
-
-    for (int s = 0; s < NIFB; ++s) {
-      const int st = s & 1;
-      const uint32_t ph = (uint32_t)(s >> 1) & 1u;
-      const int ts = s % kTStages;
-      const uint32_t tph = (uint32_t)(s / kTStages) & 1u;
-      mbar_wait(bar_t_full + 8 * ts, tph);
-      mbar_wait(bar_tm_full + 8 * st, ph);
-      tc_fence_after();
-      const float4* Ts = reinterpret_cast<const float4*>(base_ptr + (sT - base) + ts * kTBytes);
-      const float4* Bs = reinterpret_cast<const float4*>(base_ptr + (sBias - base) + ts * kBiasBytes);
-      const uint32_t tcol = tmem_base + t_lane + (uint32_t)(st * 128 + half * 16);
-      // software pipeline inside the step: the accumulator columns of (i,f) slots 2,3 are in flight while slots 0,1
-      // are contracted, so only one tcgen05.ld latency per step is exposed
-      uint32_t r[4][16];
-      tmem_ld16(tcol + 0u, r[0]);
-      tmem_ld16(tcol + 32u, r[1]);
-      tmem_ld_wait();
-      tmem_ld16(tcol + 64u, r[2]);
-      tmem_ld16(tcol + 96u, r[3]);
-#pragma unroll
-      for (int ifl = 0; ifl < 4; ++ifl) {
-        if (ifl == 2) {
-          tmem_ld_wait();
-          // every tcgen05.ld of this step has completed: hand the accumulator buffer back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_tm_empty + 8 * st);
-        }
-        float tv[PH * 4];
-#pragma unroll
-        for (int h4 = 0; h4 < PH; ++h4) {
-          const float4 t4 = Ts[(ifl * PH + h4) * 128 + el];
-          tv[h4 * 4 + 0] = t4.x; tv[h4 * 4 + 1] = t4.y; tv[h4 * 4 + 2] = t4.z; tv[h4 * 4 + 3] = t4.w;
-        }
-        unsigned long long t2[P];
-#pragma unroll
-        for (int p = 0; p < P; ++p) t2[p] = pack2(tv[p], tv[p]);
-#pragma unroll
-        for (int b4 = 0; b4 < 4; ++b4) {
-          const float4 bb = Bs[(ifl * 32 + half * 16) / 4 + b4];
-          const unsigned long long R0 = add2(pack2(__uint_as_float(r[ifl][b4 * 4 + 0]), __uint_as_float(r[ifl][b4 * 4 + 1])), pack2(bb.x, bb.y));
-          const unsigned long long R1 = add2(pack2(__uint_as_float(r[ifl][b4 * 4 + 2]), __uint_as_float(r[ifl][b4 * 4 + 3])), pack2(bb.z, bb.w));
-          if (kDumpR && s == 0 && active) {
-            float a0, a1, a2, a3;
-            unpack2(R0, a0, a1);
-            unpack2(R1, a2, a3);
-            float* dr = dumpR + (((size_t)mt * n_ob + ob) * 128 + el) * 128 + ifl * 32 + half * 16 + b4 * 4;
-            dr[0] = a0; dr[1] = a1; dr[2] = a2; dr[3] = a3;
-          }
-          if (!(dbg & 1)) {
-#pragma unroll
-            for (int p = 0; p < P; ++p) {
-              acc[b4 * 2 + 0][p] = fma2(R0, t2[p], acc[b4 * 2 + 0][p]);
-              acc[b4 * 2 + 1][p] = fma2(R1, t2[p], acc[b4 * 2 + 1][p]);
-            }
-          } else {
-            acc[b4 * 2 + 0][0] = add2(acc[b4 * 2 + 0][0], R0);
-            acc[b4 * 2 + 1][0] = add2(acc[b4 * 2 + 1][0], R1);
-          }
-        }
-      }
-      // T / bias stage fully consumed
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_t_empty + 8 * ts);
-    }
-    // write out[e, ob*32 + half*16 + (0..15), 0..P)
-    const int64_t e = mt * SE3_TILE_E + el;
-    if (active && e < E) {
-      float* dst = out + ((size_t)e * Co + (size_t)ob * SE3_TILE_O + half * 16) * P;
-#pragma unroll
-      for (int a = 0; a < 8; ++a) {
-#pragma unroll
-        for (int p = 0; p < P; ++p) {
-          float v0, v1;
-          unpack2(acc[a][p], v0, v1);
-          float* d0 = dst + (2 * a) * P + p;
-          float* d1 = dst + (2 * a + 1) * P + p;
-          if (accumulate) { v0 += *d0; v1 += *d1; }
-          *d0 = v0;
-          *d1 = v1;
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (CSZ > 1) cluster_sync_all();            // no member exits while peers may still multicast into it / arrive on its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
-  }
-}
-
-template <int P>
-static size_t tc_smem_bytes() {
-  constexpr int PH = (P + 3) / 4;
-  return 1024 + kWSlots * kUnitBytes + TStages<PH>::value * (PH * 8192u) + TStages<PH>::value * kBiasBytes + 256;
-}
-
-static int env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
-}
-
-template <int P, int CSZ, bool kDumpR>
-static int launch_tc(const TcParams& prm, cudaStream_t s) {
-  const size_t smem = tc_smem_bytes<P>();
-  auto kern = pairwise_tc_kernel<P, CSZ, kDumpR>;
-  SE3_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int n_mg = (prm.n_mt + CSZ - 1) / CSZ;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)((int64_t)n_mg * prm.n_ob * CSZ));
-  cfg.blockDim = dim3(kTcThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CSZ;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  SE3_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, prm));
-  return SE3_OK;
-}
-
-template <int P, bool kDumpR>
-static int launch_tc_csz(const TcParams& prm, int csz, cudaStream_t s) {
-  switch (csz) {
-    case 1: return launch_tc<P, 1, kDumpR>(prm, s);
-    case 4: return launch_tc<P, 4, kDumpR>(prm, s);
-    default: return launch_tc<P, 2, kDumpR>(prm, s);
-  }
-}
-
 template <bool kDumpR>
 static int dispatch_tc(const float* g, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F, int P,
                        int accumulate, float* out, float* dumpR, void* stream) {
   SE3_REQUIRE(E > 0 && Co > 0 && Ci > 0 && F > 0, "se3_pairwise_tc_fwd: bad sizes");
   SE3_REQUIRE(Co % SE3_TILE_O == 0, "se3_pairwise_tc_fwd: Co=%d must be a multiple of %d (use the SIMT kernel)", Co, SE3_TILE_O);
   SE3_REQUIRE(P == 1 || P == 3 || P == 5 || P == 7, "se3_pairwise_tc_fwd: P=%d unsupported (degree_out <= 3)", P);
-  SE3_REQUIRE((ceil_div(E, SE3_TILE_E) + 4) * (Co / SE3_TILE_O) < 2147483647ll, "se3_pairwise_tc_fwd: grid too large");
-  // tuning knobs (defaults are the shipped configuration; the env overrides exist for experiments)
-  const int dbg = env_int("SE3B200_TC_DEBUG_MODE", 0);
-  const int csz = env_int("SE3B200_TC_CLUSTER", 2);
-  const int band_m = env_int("SE3B200_TC_BANDM", 0);
-  const int band_o = env_int("SE3B200_TC_BANDO", 2);
-  TcParams prm;
-  prm.g = g;
+  SE3_REQUIRE(ceil_div(E, SE3_TILE_E) * (Co / SE3_TILE_O) < 2147483647ll, "se3_pairwise_tc_fwd: grid too large");
+  PwParams prm = {};
+  prm.A = g;
+  prm.lda = SE3_RADIAL_MID;
   prm.w_img = reinterpret_cast<const uint8_t*>(w_img);
   prm.T = T;
   prm.out = out;
   prm.dumpR = dumpR;
   prm.E = E;
-  prm.Co = Co;
   prm.NIFB = (int)ceil_div((int64_t)Ci * F, SE3_TILE_IF);
   prm.n_mt = (int)ceil_div(E, SE3_TILE_E);
   prm.n_ob = Co / SE3_TILE_O;
   prm.accumulate = accumulate;
-  prm.dbg = dbg;
-  prm.band_o = band_o > 0 ? band_o : 1;
-  const int c = (csz == 1 || csz == 4) ? csz : 2;
-  prm.band_m = band_m > 0 ? band_m : std::max(1, 148 / (c * prm.band_o));   // one wave of 148 CTAs = band_m groups x band_o blocks
+  prm.nk16 = 8;
+  prm.spu = 1;
+  prm.NU = 2 * prm.NIFB;
+  prm.out_es = (int64_t)Co * P;
+  prm.out_os = P;
+  for (int p = 0; p < 7; ++p) prm.p_off[p] = p;
   cudaStream_t s = as_stream(stream);
   switch (P) {
-    case 1: return launch_tc_csz<1, kDumpR>(prm, c, s);
-    case 3: return launch_tc_csz<3, kDumpR>(prm, c, s);
-    case 5: return launch_tc_csz<5, kDumpR>(prm, c, s);
-    default: return launch_tc_csz<7, kDumpR>(prm, c, s);
+    case 1: return launch_pw<1, true, kDumpR, 3>(prm, s);
+    case 3: return launch_pw<3, true, kDumpR, 3>(prm, s);
+    case 5: return launch_pw<5, true, kDumpR, 3>(prm, s);
+    default: return launch_pw<7, true, kDumpR, 3>(prm, s);
   }
 }
 

@@ -2,8 +2,8 @@
 // (degree_in, degree_out) pairs of one ConvSE3 in a single launch.  The last Linear (net.6) is NOT applied here:
 // its output is consumed on-chip by the pairwise kernels.
 //
-// Output: g fp32 [pairs, E, 128]; the tensor-core kernel splits its 128-edge tile of g into bf16 hi/lo on the fly
-// while loading it into tensor memory.
+// Output: g fp32 [pairs, E, 128]; the tensor-core kernel splits its 128-edge tile of g into fp16 hi/lo on the fly
+// while loading it into shared memory.
 #include "common.cuh"
 
 namespace se3 {

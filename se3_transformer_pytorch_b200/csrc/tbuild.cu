@@ -160,8 +160,8 @@ extern "C" int se3_tbuild_fwd(const float* x, const int64_t* idx, const float* b
   const int64_t n_all = ceil_div(E, kTE);
   SE3_REQUIRE(tile_begin >= 0 && tile_count > 0 && tile_begin + tile_count <= n_all, "se3_tbuild_fwd: tile range out of bounds");
   const int64_t n_mtiles = tile_count;
-  // enough CTAs to fill the machine (148 SMs x a few CTAs) without shredding the channel loop
-  int slabs = (int)std::min<int64_t>(std::max(1, Ci / 16), std::max<int64_t>(1, (148 * 2 + n_mtiles - 1) / n_mtiles));
+  // enough CTAs to fill the machine (132 SMs x a few CTAs) without shredding the channel loop
+  int slabs = (int)std::min<int64_t>(std::max(1, Ci / 16), std::max<int64_t>(1, (132 * 2 + n_mtiles - 1) / n_mtiles));
   const int ci_per_cta = (int)ceil_div(Ci, slabs);
   slabs = (int)ceil_div(Ci, ci_per_cta);
   dim3 grid((unsigned)n_mtiles, (unsigned)slabs);

@@ -7,42 +7,35 @@
 //              out'[e,o,-] = sum_{li>=m} sum_i  b[e,o,i] x'[e,i,+m] + a[e,o,i] x'[e,i,-m]
 // (reference S:237-254, 326-343 re-associated), and every radial weight is a short dot product with the per-edge radial
 // coordinates U of its degree pair, w[e,o,i] = sum_k U[e,k] F'[(o,i),k] (DESIGN.md 4.2; K = r+1 <= 16 per sub-segment).
-// Instead of forming w (R-first: a K = 16 GEMM per radial weight tile, then 2 fp32 FMAs per weight on the SIMT pipe, a TMEM
-// read of every weight and a hand-off per tile) the sums are exchanged:
+// Instead of forming w the sums are exchanged:
 //     out'[e,o,c] = sum_{(li,i,f,k)}  Z_c[e,(li,i,f,k)] * F'[o,(li,i,f,k)],        Z_c[e,(li,i,f,k)] = +-U_li[e,k] x'_li[e,i,+-m]
 // one GEMM with M = edges, N = output channels, K = sum_li C_in * F * 16, whose A operand Z is an outer product per edge:
 // it costs E*C_in*16 multiplies to make (C_out times fewer than there are radial weights) and is produced by the CUDA cores
-// straight into tensor memory, split x = hi + lo in fp16 for the 3-pass fp32-parity MMA (hi*hi + lo*hi + hi*lo).  The
-// accumulator stays in tensor memory over the whole K loop; nothing per radial weight ever touches the SIMT pipe.
+// straight into the A-operand registers of wgmma, split z = hi + lo in fp16 for the 3-pass fp32-parity MMA
+// (hi*hi + lo*hi + hi*lo).  Nothing per radial weight ever touches the SIMT pipe.
 //
 // MODE 3 evaluates the |m| > 0 case with three real products per complex one (Gauss): with c = x'[+m], d = x'[-m],
 //     S1 = sum (a+b) c,   S2 = sum a (d-c),   S3 = sum b (c+d);    out'[+] = S1 - S3,   out'[-] = S1 + S2
 // i.e. three accumulators, each fed by its own weight set (a+b, a, b) and its own Z: 3 instead of 4 K = 16 GEMM units per
-// (edge, o, i).  Stages cycle through the three sets (4 input channels per stage); the drain combines them.
+// (edge, o, i).  Chunk c of stage s belongs to weight set (4 s + c) % 3; the drain combines them.
 //
-// CTA = 128 edges x N channels (MODE 1: one component, N = 256 or 128; MODE 2: components (+m, -m), N = 128, two
-// accumulators fed by the same B tiles).  384 threads: warp 0 streams the weight image (TMA bulk copies, 2-CTA multicast),
-// warp 1 issues tcgen05.mma (.ts form: A from tensor memory), warps 4-11 generate Z (one warp per TMEM lane quarter and stage
-// parity) and own the fp32 partial sums: tensor-core accumulation rounds toward zero, so every `flush_stages` stages the
-// accumulator is drained into registers (round-to-nearest adds) and restarted.
+// CTA = 128 edges x NC channels (a slice of an N-wide tile of the weight image; MODE 1 / 4: NC = 128, one accumulator;
+// MODE 2: NC = 64, components (+m, -m) in two accumulators fed by the same B tiles; MODE 3: NC = 64, three accumulators).
+// 384 threads: warp 0 streams the weight image (TMA bulk copies into an mbarrier ring); warpgroups 1 and 2 own 64 edge rows
+// each, generate Z for their rows, issue m64 x NC x 16 wgmma with A from registers and B from shared memory, and keep the
+// fp32 partial sums: tensor-core accumulation truncates, so every `flush_stages` stages the accumulators are added into
+// registers with round-to-nearest adds and restarted.  The two warpgroups interleave, so one's MMAs overlap the other's
+// generation.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 namespace se3 {
 
-// timing experiments only (results are wrong): move only 1 / SE3_Z_DBG_WDIV of every weight stage (how much of the power budget
-// does the L2 -> shared-memory weight stream take?)
-#ifndef SE3_Z_DBG_WDIV
-#define SE3_Z_DBG_WDIV 1
-#endif
-#ifndef SE3_Z_ISSUERS3
-#define SE3_Z_ISSUERS3 1
-#endif
 constexpr int kZThreads = 384;
 constexpr int kZMaxSeg = 16;
-constexpr uint32_t kZTmemCols = 512;
 constexpr uint32_t kZWRingBytes = 196608;     // shared memory for the weight ring
 
 struct ZSeg {
@@ -63,504 +56,311 @@ struct ZParams {
   int n_mt, n_nt, S, flush_stages;
 };
 
-__device__ __forceinline__ void z_split16(const float (&p)[16], uint32_t (&r)[16]) {
-  // 16 fp32 -> 8 packed fp16 pairs hi (r[0..7]) + 8 packed pairs lo (r[8..15]); element 2c in the low half
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const __half2 h = __floats2half2_rn(p[2 * c], p[2 * c + 1]);
-    const float2 hf = __half22float2(h);
-    const __half2 l = __floats2half2_rn(p[2 * c] - hf.x, p[2 * c + 1] - hf.y);
-    r[c] = *reinterpret_cast<const uint32_t*>(&h);
-    r[8 + c] = *reinterpret_cast<const uint32_t*>(&l);
+// A fragment of one K = 16 chunk for rows (r0, r0 + 8), columns (kq, kq+1, kq+8, kq+9): v[row][4] -> fp16 hi / lo pairs
+__device__ __forceinline__ void z_frag(const float (&v)[2][4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+  split_h2(v[0][0], v[0][1], hi[0], lo[0]);
+  split_h2(v[1][0], v[1][1], hi[1], lo[1]);
+  split_h2(v[0][2], v[0][3], hi[2], lo[2]);
+  split_h2(v[1][2], v[1][3], hi[3], lo[3]);
+}
+
+template <int NR>
+__device__ __forceinline__ void z_mma3(float (&d)[NR], const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint64_t b_hi, uint64_t b_lo) {
+  if constexpr (NR == 64) {
+    wgmma_rs_n128(d, hi, b_hi);
+    wgmma_rs_n128(d, lo, b_hi);
+    wgmma_rs_n128(d, hi, b_lo);
+  } else {
+    wgmma_rs_n64(d, hi, b_hi);
+    wgmma_rs_n64(d, lo, b_hi);
+    wgmma_rs_n64(d, hi, b_lo);
   }
 }
 
-// Z = U * y for 16 radial coordinates and one scalar y, as fp16 pairs hi (r[0..7]) + lo (r[8..15]) with hi + lo = U y to ~2^-22,
-// entirely in packed half arithmetic (4 instructions per pair of values, no conversions): with U = Uh + Ul, y = yh + yl,
-//     hi = fl(Uh yh);   e = fma(Uh, yh, -hi)  (the rounding error of that product, exact: TwoProduct);   lo = Uh yl + (Ul yh + e)
-// (Ul yl ~ 2^-22 is dropped).  Uh / Ul: the segment's radial coordinates, split once per segment.
-__device__ __forceinline__ void z_outer16(const __half2 (&Uh)[8], const __half2 (&Ul)[8], float y, uint32_t (&r)[16]) {
-  const __half yh1 = __float2half_rn(y);
-  const __half yl1 = __float2half_rn(y - __half2float(yh1));
-  const __half2 yh = __half2half2(yh1), yl = __half2half2(yl1);
-#pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const __half2 hi = __hmul2(Uh[c], yh);
-    const __half2 e = __hfma2(Uh[c], yh, __hneg2(hi));
-    const __half2 lo = __hfma2(Uh[c], yl, __hfma2(Ul[c], yh, e));
-    r[c] = *reinterpret_cast<const uint32_t*>(&hi);
-    r[8 + c] = *reinterpret_cast<const uint32_t*>(&lo);
-  }
-}
-
-template <bool PAIR>
-__device__ __forceinline__ void z_mma(uint32_t d, uint32_t a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (PAIR) tc_mma_f16_ts_pair(d, a, bdesc, idesc, accumulate);
-  else tc_mma_f16_ts(d, a, bdesc, idesc, accumulate);
-}
-
-template <int MODE, int N, int CSZ, bool PAIR = false>
+template <int MODE, int N, int NC>
 __global__ void __launch_bounds__(kZThreads, 1)
 zgemm_kernel(const __grid_constant__ ZParams prm) {
-  // PAIR: the two CTAs of the cluster (neighbouring edge tiles of one channel tile) run as ONE tensor-core pair (cta_group::2):
-  // the leader's MMA covers M = 256 = both edge tiles, each CTA streams only ITS half of every weight stage (rows r N/2 ..) into
-  // its own shared memory -- half the L2 -> shared-memory weight traffic per SM, which costs 15 % of the kernel's time through
-  // the power cap (DESIGN.md section 6).  Generators, accumulators and drains stay per CTA.
-  static_assert(!PAIR || (CSZ == 2 && (MODE == 1 || MODE == 3)), "pair mode: 2-CTA cluster, MODE 1 / 3");
-  static_assert(MODE == 1 || ((MODE == 2 || MODE == 3 || MODE == 4) && N == 128), "MODE 2 / 3 use two / three N = 128 accumulators");
-  constexpr int DCOLS = (MODE == 3) ? 384 : (MODE == 2) ? 256 : N;   // accumulator columns in use
-  constexpr int ACC = (MODE == 3) ? 128 : DCOLS / 2;      // fp32 partial sums per drain thread (MODE 3: 64 of out'[+], 64 of out'[-])
-  constexpr int ASLOT = (MODE == 2) ? 128 : 64;           // TMEM columns of one A stage
-  constexpr uint32_t kZACol = (MODE == 3) ? 384 : 256;    // D: columns [0, kZACol); A ring: columns [kZACol, 512)
-  constexpr int AS = (512 - (int)kZACol) / ASLOT;         // A ring depth (stages)
-  constexpr uint32_t kImgStage = 2u * N * 128u;            // one stage of the weight image: [hi N rows | lo N rows] x 128 B
-  constexpr uint32_t kStageBytes = PAIR ? kImgStage / 2 : kImgStage;      // what one CTA keeps of it in shared memory
-  constexpr uint32_t kLoOff = PAIR ? (N / 2) * 128u : N * 128u;           // lo part inside a shared-memory stage
-  constexpr int WS = (kZWRingBytes / kStageBytes > 8) ? 8 : (int)(kZWRingBytes / kStageBytes);     // W ring depth (stages)
-  constexpr uint32_t kIdesc = (1u << 4) | ((uint32_t)(N >> 3) << 17) | (((PAIR ? 256u : 128u) >> 4) << 24);
-  constexpr uint16_t kMask = (uint16_t)((1u << CSZ) - 1u);
-  // MMA-issuing warps.  One thread issues an N = 128 tcgen05.mma only every ~85 cycles (measured: 72 % tensor-pipe utilisation in
-  // MODE 3 whatever the generators do, 92 % in MODE 1 whose N = 256 instructions last 128 cycles), so MODE 3 uses three issuers,
-  // warps 1-3, one per accumulator / weight set; every hand-off barrier then counts three commits.
-  constexpr int NI = (MODE == 3 && SE3_Z_ISSUERS3) ? 3 : 1;
+  static_assert((MODE == 1 || MODE == 4) ? NC == 128 : NC == 64, "CTA width");
+  static_assert(N % NC == 0 && (MODE == 1 || N == 128), "weight image tile");
+  constexpr int NA = (MODE == 3) ? 3 : (MODE == 2) ? 2 : 1;   // accumulators
+  constexpr int NO = (MODE == 2 || MODE == 3) ? 2 : 1;        // output planes
+  constexpr int NR = NC / 2;                                   // fragment registers of one m64 x NC fp32 accumulator
+  constexpr int NH = N / NC;                                   // CTAs per tile of the weight image
+  constexpr uint32_t kImgStage = 2u * N * 128u;                // one stage of the weight image: [hi N rows | lo N rows] x 128 B
+  constexpr uint32_t kStageBytes = 2u * NC * 128u;             // what one CTA keeps of it: its NC rows of hi and of lo
+  constexpr int WS = (kZWRingBytes / kStageBytes > 8) ? 8 : (int)(kZWRingBytes / kStageBytes);
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - raw);
   const uint32_t sW = base;
-  const uint32_t sBar = sW + WS * kStageBytes;
-  const uint32_t bar_w_full = sBar;
+  const uint32_t bar_w_full = sW + WS * kStageBytes;
   const uint32_t bar_w_empty = bar_w_full + 8 * WS;
-  const uint32_t bar_a_full = bar_w_empty + 8 * WS;
-  const uint32_t bar_a_empty = bar_a_full + 8 * AS;
-  const uint32_t bar_d_full = bar_a_empty + 8 * AS;
-  const uint32_t bar_d_empty = bar_d_full + 8;
-  const uint32_t bar_peer_w = bar_d_empty + 8;            // [WS] (pair mode, leader): the peer's half of a weight stage is in place
-  const uint32_t s_tmem_slot = bar_peer_w + 8 * WS;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + (s_tmem_slot - base));
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const uint32_t crank = (CSZ > 1) ? cluster_ctarank() : 0u;
   const int S = prm.S, FS = prm.flush_stages;
-  // cluster = CSZ consecutive edge tiles of one channel tile (they share every weight stage); channel tile fastest
-  const int64_t cid = blockIdx.x / CSZ;
-  const int nt = (int)(cid % prm.n_nt);
-  int64_t mt = (cid / prm.n_nt) * CSZ + crank;
-  const bool active = mt < prm.n_mt;
-  if (!active) mt = prm.n_mt - 1;
+  const int n_ct = prm.n_nt * NH;
+  const int ctile = (int)(blockIdx.x % n_ct);
+  const int64_t mt = blockIdx.x / n_ct;
+  const int nt = ctile / NH, hs = ctile % NH;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < WS; ++s) {
       mbar_init(bar_w_full + 8 * s, 1);
-      mbar_init(bar_w_empty + 8 * s, PAIR ? NI : CSZ * NI);
+      mbar_init(bar_w_empty + 8 * s, 8);       // one arrival per consumer warp
     }
-    for (int s = 0; s < AS; ++s) {
-      mbar_init(bar_a_full + 8 * s, PAIR ? 8 : 4);           // pair mode: the generators of both CTAs report to the leader
-      mbar_init(bar_a_empty + 8 * s, NI);
-    }
-    mbar_init(bar_d_full, NI);
-    mbar_init(bar_d_empty, PAIR ? 16 : 8);                 // pair mode: the drain warps of both CTAs report to the leader
-    for (int s = 0; s < WS; ++s) mbar_init(bar_peer_w + 8 * s, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    if (PAIR) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_tmem_slot), "r"(kZTmemCols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_tmem_slot), "r"(kZTmemCols) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if (CSZ > 1) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
 
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (warp == 0) {
+    if (warp == 0 && lane == 0) {
       // ===================== weight producer =====================
-      const uint8_t* wsrc = prm.w_img + (size_t)nt * S * kImgStage;
-      constexpr uint32_t kMove = kStageBytes / SE3_Z_DBG_WDIV;
-      constexpr uint32_t kShare = kMove / CSZ;
+      const uint8_t* wsrc = prm.w_img + (size_t)nt * S * kImgStage + (size_t)hs * NC * 128u;
       for (int s = 0; s < S; ++s) {
         const int slot = s % WS;
-        const uint32_t ph = (uint32_t)(s / WS) & 1u;
-        mbar_wait(bar_w_empty + 8 * slot, ph ^ 1u);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(bar_w_full + 8 * slot, kMove);
-          if (PAIR) {
-            // this CTA's rows [crank N/2, +N/2) of the hi and of the lo part
-            constexpr uint32_t kHalf = (N / 2) * 128u / SE3_Z_DBG_WDIV;
-            const uint8_t* src = wsrc + (size_t)s * kImgStage + crank * (N / 2) * 128u;
-            bulk_g2s(sW + slot * kStageBytes, src, kHalf, bar_w_full + 8 * slot);
-            bulk_g2s(sW + slot * kStageBytes + kLoOff, src + N * 128u, kHalf, bar_w_full + 8 * slot);
-          } else if (CSZ == 1) {
-            bulk_g2s(sW + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kMove, bar_w_full + 8 * slot);
-          } else {
-            bulk_g2s_mc(sW + slot * kStageBytes + crank * kShare, wsrc + (size_t)s * kStageBytes + crank * kShare, kShare,
-                        bar_w_full + 8 * slot, kMask);
-          }
-        }
-        __syncwarp();
+        mbar_wait(bar_w_empty + 8 * slot, ((uint32_t)(s / WS) & 1u) ^ 1u);
+        mbar_arrive_expect_tx(bar_w_full + 8 * slot, kStageBytes);
+        bulk_g2s(sW + slot * kStageBytes, wsrc + (size_t)s * kImgStage, NC * 128u, bar_w_full + 8 * slot);
+        bulk_g2s(sW + slot * kStageBytes + NC * 128u, wsrc + (size_t)s * kImgStage + N * 128u, NC * 128u, bar_w_full + 8 * slot);
       }
-    } else if (PAIR && crank != 0) {
-      // ===================== pair mode, peer CTA: tell the leader when my half of a weight stage has landed =====================
-      // (the weight ring runs many stages ahead, so this relay is off the critical path; the generators of this CTA arrive on the
-      // leader's A-stage barrier themselves)
-      if (warp == 1) {
-        for (int s = 0; s < S; ++s) {
-          mbar_wait(bar_w_full + 8 * (s % WS), (uint32_t)(s / WS) & 1u);
-          if (elect_one()) mbar_arrive_remote(bar_peer_w + 8 * (s % WS), 0u);
-          __syncwarp();
+    }
+    return;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  // ===================== Z generators + MMA + fp32 partial sums =====================
+  const int ct = threadIdx.x - 128;
+  const int r0 = (ct >> 7) * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);    // rows r0, r0 + 8 of the edge tile
+  const int kq = 2 * (lane & 3);                                         // columns kq, kq+1, kq+8, kq+9 of every K chunk
+  int64_t eg[2];
+  bool live[2];
+  float sxe[2];
+#pragma unroll
+  for (int rs = 0; rs < 2; ++rs) {
+    eg[rs] = mt * SE3_TILE_E + r0 + 8 * rs;
+    live[rs] = eg[rs] < prm.E;
+    sxe[rs] = (live[rs] && MODE != 4) ? prm.sx[eg[rs]] : 1.f;
+  }
+  float D[NA][NR], acc[NO][NR];
+#pragma unroll
+  for (int a = 0; a < NA; ++a)
+#pragma unroll
+    for (int j = 0; j < NR; ++j) D[a][j] = 0.f;
+#pragma unroll
+  for (int a = 0; a < NO; ++a)
+#pragma unroll
+    for (int j = 0; j < NR; ++j) acc[a][j] = 0.f;
+  int blk_start = 0;
+
+  // after stage s: hand the weight slot back, drain the accumulators at the end of a block
+  auto finish_stage = [&](int s) {
+    wgmma_commit();
+    wgmma_wait0();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_w_empty + 8 * (s % WS));
+    if (s + 1 == S || s + 1 - blk_start == FS) {
+#pragma unroll
+      for (int j = 0; j < NR; ++j) {
+        if (MODE == 3) {
+          acc[0][j] += D[0][j] - D[NA - 1][j];
+          acc[1][j] += D[0][j] + D[NA > 1 ? 1 : 0][j];
+        } else {
+#pragma unroll
+          for (int a = 0; a < NA; ++a) acc[a][j] += D[a][j];
         }
+#pragma unroll
+        for (int a = 0; a < NA; ++a) D[a][j] = 0.f;
       }
-    } else if (warp == 1 || (NI == 3 && warp <= 3)) {
-      // ===================== MMA issuer(s) =====================
-      const int my_ty = warp - 1;                   // NI == 3: the accumulator (weight set) this warp feeds
-      int blk_start = 0, blk = 0;
-      for (int s = 0; s < S; ++s) {
-        const int wslot = s % WS, aslot = s % AS;
-        if (s == blk_start && blk > 0) {
-          mbar_wait(bar_d_empty, (uint32_t)(blk - 1) & 1u);          // the previous block has been drained into registers
-        }
-        mbar_wait(bar_w_full + 8 * wslot, (uint32_t)(s / WS) & 1u);
-        mbar_wait(bar_a_full + 8 * aslot, (uint32_t)(s / AS) & 1u);
-        if (PAIR) mbar_wait(bar_peer_w + 8 * wslot, (uint32_t)(s / WS) & 1u);
-        tc_fence_after();
-        const uint32_t wb = sW + wslot * kStageBytes;
-        const bool last_of_blk = (s + 1 == S) || (s + 1 == blk_start + FS);
-        if (elect_one()) {
-          if (MODE == 1 || MODE == 4) {
-            uint32_t accum = (s == blk_start) ? 0u : 1u;
+      blk_start = s + 1;
+    }
+  };
+  auto wait_stage = [&](int s, uint64_t& b_hi, uint64_t& b_lo) {
+    mbar_wait(bar_w_full + 8 * (s % WS), (uint32_t)(s / WS) & 1u);
+    const uint32_t wb = sW + (uint32_t)(s % WS) * kStageBytes;
+    b_hi = wg_desc_sw128(wb);
+    b_lo = wg_desc_sw128(wb + NC * 128u);
+  };
+
+  if constexpr (MODE == 4) {
+    // ---- LinearSE3 (reference S:78-95): rows = (node, m) of x [nodes, D, M], A[row, d] = x[node, d, m] read in place (stride
+    // M), chunk c of stage s = input channels 64 s + 16 c .. +15; out[node, o, m] (+ residual) in the reference layout
+    const ZSeg& z = prm.seg[0];
+    const int M = z.ncomp, Dn = z.Ci;
+    int64_t node[2];
+    int m[2];
+    float sc[2];
+    const float* xrow[2];
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const uint32_t a_hi = tmem_base + kZACol + (uint32_t)(aslot * ASLOT + c * 16);
-              const uint64_t b_hi = umma_desc_sw128(wb + c * 32);
-              const uint64_t b_lo = umma_desc_sw128(wb + kLoOff + c * 32);
-              z_mma<PAIR>(tmem_base, a_hi, b_hi, kIdesc, accum);
-              z_mma<PAIR>(tmem_base, a_hi + 8, b_hi, kIdesc, 1u);
-              z_mma<PAIR>(tmem_base, a_hi, b_lo, kIdesc, 1u);
-              accum = 1u;
-            }
-          } else if (MODE == 3) {
-            // chunk c of stage s belongs to weight set (s + c) % 3 (every segment has a multiple of 3 stages)
-            if (NI == 3) {
-              // this issuer: the chunks of ITS set, (c - my_ty + s) % 3 == 0 -> c0 = (my_ty - s) mod 3, and c0 + 3 if that is 3
-              const int c0 = ((my_ty - s) % 3 + 3) % 3;
-              uint32_t accum = (s == blk_start) ? 0u : 1u;
-              const uint32_t d = tmem_base + (uint32_t)(my_ty * 128);
-              for (int c = c0; c < 4; c += 3) {
-                const uint32_t a_hi = tmem_base + kZACol + (uint32_t)(aslot * ASLOT + c * 16);
-                const uint64_t b_hi = umma_desc_sw128(wb + c * 32);
-                const uint64_t b_lo = umma_desc_sw128(wb + kLoOff + c * 32);
-                z_mma<PAIR>(d, a_hi, b_hi, kIdesc, accum);
-                z_mma<PAIR>(d, a_hi + 8, b_hi, kIdesc, 1u);
-                z_mma<PAIR>(d, a_hi, b_lo, kIdesc, 1u);
-                accum = 1u;
-              }
-            } else {
-              // one issuer, pass-major order: consecutive MMAs hit S1, S2, S3, S1' in turn
-              const int blk_first = (s == blk_start);
+    for (int rs = 0; rs < 2; ++rs) {
+      node[rs] = live[rs] ? eg[rs] / M : 0;
+      m[rs] = live[rs] ? (int)(eg[rs] - node[rs] * M) : 0;
+      sc[rs] = live[rs] ? prm.sx[node[rs]] : 1.f;
+      xrow[rs] = z.X + ((size_t)node[rs] * Dn) * M + m[rs];
+    }
+    for (int s = 0; s < S; ++s) {
+      float v[4][2][4];
 #pragma unroll
-              for (int pass = 0; pass < 3; ++pass) {
+      for (int c = 0; c < 4; ++c)
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                  const int ty = (s + c) % 3;
-                  const uint32_t d = tmem_base + (uint32_t)(ty * 128);
-                  const uint32_t a_hi = tmem_base + kZACol + (uint32_t)(aslot * ASLOT + c * 16);
-                  const uint64_t b_hi = umma_desc_sw128(wb + c * 32);
-                  const uint64_t b_lo = umma_desc_sw128(wb + kLoOff + c * 32);
-                  const uint32_t accum = (blk_first && pass == 0 && c < 3) ? 0u : 1u;
-                  z_mma<PAIR>(d, pass == 1 ? a_hi + 8 : a_hi, pass == 2 ? b_lo : b_hi, kIdesc, accum);
-                }
-              }
-            }
-          } else {
+        for (int rs = 0; rs < 2; ++rs)
 #pragma unroll
-            for (int comp = 0; comp < 2; ++comp) {
-              uint32_t accum = (s == blk_start) ? 0u : 1u;
-#pragma unroll
-              for (int c = 0; c < 4; ++c) {
-                const uint32_t a_hi = tmem_base + kZACol + (uint32_t)(aslot * ASLOT + comp * 64 + c * 16);
-                const uint64_t b_hi = umma_desc_sw128(wb + c * 32);
-                const uint64_t b_lo = umma_desc_sw128(wb + kLoOff + c * 32);
-                const uint32_t d = tmem_base + (uint32_t)(comp * 128);
-                z_mma<PAIR>(d, a_hi, b_hi, kIdesc, accum);
-                z_mma<PAIR>(d, a_hi + 8, b_hi, kIdesc, 1u);
-                z_mma<PAIR>(d, a_hi, b_lo, kIdesc, 1u);
-                accum = 1u;
-              }
-            }
+          for (int q = 0; q < 4; ++q) {
+            const int d = 64 * s + 16 * c + kq + (q & 1) + 8 * (q >> 1);
+            v[c][rs][q] = live[rs] ? __ldg(xrow[rs] + (size_t)d * M) * sc[rs] : 0.f;
           }
-          if (PAIR) {                        // one commit per barrier, multicast to both CTAs of the pair
-            tc_commit_pair(bar_w_empty + 8 * wslot, kMask);
-            tc_commit_pair(bar_a_empty + 8 * aslot, kMask);
-            if (last_of_blk) tc_commit_pair(bar_d_full, kMask);
-          } else {
-            if (CSZ == 1) tc_commit(bar_w_empty + 8 * wslot);
-            else tc_commit_mc(bar_w_empty + 8 * wslot, kMask);
-            tc_commit(bar_a_empty + 8 * aslot);
-            if (last_of_blk) tc_commit(bar_d_full);
-          }
+      uint64_t b_hi, b_lo;
+      wait_stage(s, b_hi, b_lo);
+      uint32_t hi[4][4], lo[4][4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) z_frag(v[c], hi[c], lo[c]);
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < 4; ++c) z_mma3<NR>(D[0], hi[c], lo[c], b_hi + 2 * c, b_lo + 2 * c);
+      finish_stage(s);
+    }
+#pragma unroll
+    for (int rs = 0; rs < 2; ++rs) {
+      if (!live[rs]) continue;
+      const float inv = 1.f / sc[rs];
+      const int64_t Eo = prm.out_es;                            // output channels of the layer
+      const size_t o0 = (size_t)nt * N + (size_t)hs * NC + kq;
+      float* dst = prm.out + ((size_t)node[rs] * Eo + o0) * M + m[rs];
+      const float* res = z.U ? z.U + ((size_t)node[rs] * Eo + o0) * M + m[rs] : nullptr;
+#pragma unroll
+      for (int g = 0; g < NC / 8; ++g)
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+          const size_t o = (size_t)(8 * g + b) * M;
+          dst[o] = acc[0][4 * g + 2 * rs + b] * inv + (res ? __ldg(res + o) : 0.f);
         }
-        __syncwarp();
-        if (last_of_blk) { blk_start = s + 1; ++blk; }
-      }
     }
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-    // ===================== Z generators + fp32 partial sums =====================
-    const int q = warp & 3;                    // TMEM lane quarter
-    const int h = (warp - 4) >> 2;             // stage parity generated by this warp / accumulator half drained by it
-    const int el = q * 32 + lane;
-    const uint32_t t_lane = ((uint32_t)(q * 32)) << 16;
-    const int64_t eg = mt * SE3_TILE_E + el;
-    const bool live = eg < prm.E;
-    const float sxe = (live && MODE != 4) ? prm.sx[eg] : 1.f;
-
-    float acc[ACC];
-#pragma unroll
-    for (int j = 0; j < ACC; ++j) acc[j] = 0.f;
-    int flushed = 0;                           // accumulation blocks drained so far
-    const int n_blk = (S + FS - 1) / FS;
-
-    auto drain = [&]() {
-      mbar_wait(bar_d_full, (uint32_t)flushed & 1u);
-      tc_fence_after();
-      if (MODE == 3) {
-        // channels h*64 .. h*64+63 of the three sets: out'[+] += S1 - S3, out'[-] += S1 + S2
-        constexpr bool has1 = true, has2 = true, has3 = true;      // every stage feeds all three sets
-        const uint32_t c0 = tmem_base + t_lane + (uint32_t)(h * 64);
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          uint32_t r1[16], r2[16], r3[16];
-          tmem_ld16(c0 + (uint32_t)(t * 16), r1);
-          tmem_ld16(c0 + 128u + (uint32_t)(t * 16), r2);
-          tmem_ld16(c0 + 256u + (uint32_t)(t * 16), r3);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float s1 = has1 ? __uint_as_float(r1[j]) : 0.f, s2 = has2 ? __uint_as_float(r2[j]) : 0.f, s3 = has3 ? __uint_as_float(r3[j]) : 0.f;
-            acc[t * 16 + j] += s1 - s3;
-            acc[64 + t * 16 + j] += s1 + s2;
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { if (PAIR && crank != 0) mbar_arrive_remote(bar_d_empty, 0u); else mbar_arrive(bar_d_empty); }
-        ++flushed;
-        return;
-      }
-      const uint32_t c0 = tmem_base + t_lane + (uint32_t)(h * ACC);
-#pragma unroll
-      for (int t = 0; t < ACC / 32; ++t) {
-        uint32_t ra[16], rb[16];
-        tmem_ld16(c0 + (uint32_t)(t * 32), ra);
-        tmem_ld16(c0 + (uint32_t)(t * 32 + 16), rb);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          acc[t * 32 + j] += __uint_as_float(ra[j]);
-          acc[t * 32 + 16 + j] += __uint_as_float(rb[j]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { if (PAIR && crank != 0) mbar_arrive_remote(bar_d_empty, 0u); else mbar_arrive(bar_d_empty); }
-      ++flushed;
-    };
-
-    if (MODE == 4) {
-      // ---- LinearSE3 (reference S:78-95): rows = (node, m) of x [nodes, D, M], A[row, d] = x[node, d, m] read in place (stride
-      // M), chunk c of stage s = input channels 64 s + 16 c .. +15; out[node, o, m] (+ residual) in the reference layout
-      const ZSeg& z = prm.seg[0];
-      const int M = z.ncomp, D = z.Ci;
-      const int64_t node = live ? eg / M : 0;
-      const int m = live ? (int)(eg - node * M) : 0;
-      const float sc = live ? prm.sx[node] : 1.f;
-      const float* xrow = z.X + ((size_t)node * D) * M + m;
-      float xa[32], xb[32];
-      auto ldhalf = [&](int st, int half, float (&dst)[32]) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) dst[j] = live ? __ldg(xrow + (size_t)(st * 64 + half * 32 + j) * M) : 0.f;
-      };
-      auto gen2 = [&](const float (&src)[32], uint32_t a0) {
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          float p[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) p[j] = src[c * 16 + j] * sc;
-          uint32_t r[16];
-          z_split16(p, r);
-          tmem_st16(a0 + (uint32_t)(c * 16), r);
-        }
-      };
-      int s = h;
-      if (s < S) ldhalf(s, 0, xa);
-      for (; s < S; s += 2) {
-        ldhalf(s, 1, xb);
-        while (flushed < n_blk && min((flushed + 1) * FS, S) - 1 <= s - AS) drain();
-        const int aslot = s % AS;
-        mbar_wait(bar_a_empty + 8 * aslot, ((uint32_t)(s / AS) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t a0 = tmem_base + t_lane + kZACol + (uint32_t)(aslot * ASLOT);
-        gen2(xa, a0);
-        if (s + 2 < S) ldhalf(s + 2, 0, xa);
-        gen2(xb, a0 + 32u);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_a_full + 8 * aslot);
-      }
-      while (flushed < n_blk) drain();
-      if (active && live) {
-        const float inv = 1.f / sc;
-        const int64_t Eo = prm.out_es;                            // output channels of the layer
-        const size_t o0 = (size_t)nt * N + h * ACC;
-        float* dst = prm.out + ((size_t)node * Eo + o0) * M + m;
-        const float* res = z.U ? z.U + ((size_t)node * Eo + o0) * M + m : nullptr;
-#pragma unroll
-        for (int j = 0; j < ACC; ++j) dst[(size_t)j * M] = acc[j] * inv + (res ? __ldg(res + (size_t)j * M) : 0.f);
-      }
-    } else {
-    // ---- generators of MODE 1 / 2 / 3: warp h fills the stages of parity h.  Lean loop: the segment's constants live in
-    // registers, positions are running counters (ncu r02b: 391 instructions per stage of which only 128 were the outer product;
-    // the generation latency of a stage, not the tensor pipe, bounded MODE 3)
-    __half2 Uh[8], Ul[8];                      // the segment's radial coordinates U[e, 0..15], split hi / lo
-    constexpr int NX = (MODE == 1) ? 4 : 8;
-    constexpr int LOG_AS = (AS == 4) ? 2 : 1;
-    static_assert(AS == (1 << LOG_AS), "A ring depth");
-    int s0 = 0;                                // global index of the current segment's first stage
-    int next_drain = min(FS, S) - 1 + AS;      // block `flushed` is drained before generating a stage s >= next_drain
+    // ---- MODE 1 / 2 / 3
+    int s = 0;                                 // global stage index
     for (int sg = 0; sg < prm.n_seg; ++sg) {
-      const int ns = prm.seg[sg].n_stage, ncomp = prm.seg[sg].ncomp;
-      const size_t istride = (size_t)ncomp * 128;                       // floats between consecutive input channels of X
-      const float* xp = prm.seg[sg].X + ((size_t)mt * prm.seg[sg].Ci * ncomp + prm.seg[sg].cplus) * 128 + el;
-      const float* xm = prm.seg[sg].X + ((size_t)mt * prm.seg[sg].Ci * ncomp + prm.seg[sg].cminus) * 128 + el;
-      {
-        const float4* urow = reinterpret_cast<const float4*>(prm.seg[sg].U + (size_t)(live ? eg : 0) * 64);
+      const ZSeg& z = prm.seg[sg];
+      const int ns = z.n_stage;
+      const size_t istride = (size_t)z.ncomp * 128;                     // floats between consecutive input channels of X
+      const float* xp = z.X + ((size_t)mt * z.Ci * z.ncomp + z.cplus) * 128 + r0;
+      const float* xm = z.X + ((size_t)mt * z.Ci * z.ncomp + z.cminus) * 128 + r0;
+      float u[2][4];                           // U[e, kq, kq+1, kq+8, kq+9] * sx[e] of rows r0, r0 + 8
 #pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          const float4 u4 = live ? __ldg(urow + v) : make_float4(0.f, 0.f, 0.f, 0.f);
-          const __half2 h0 = __floats2half2_rn(u4.x, u4.y), h1 = __floats2half2_rn(u4.z, u4.w);
-          const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-          Uh[2 * v] = h0; Uh[2 * v + 1] = h1;
-          Ul[2 * v] = __floats2half2_rn(u4.x - f0.x, u4.y - f0.y);
-          Ul[2 * v + 1] = __floats2half2_rn(u4.z - f1.x, u4.w - f1.y);
-        }
+      for (int rs = 0; rs < 2; ++rs) {
+        const float* urow = z.U + (size_t)(live[rs] ? eg[rs] : 0) * 64;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) u[rs][q] = live[rs] ? __ldg(urow + kq + (q & 1) + 8 * (q >> 1)) * sxe[rs] : 0.f;
       }
-      // raw loads only (MODE 3: combining x+ / x- at load time would wait for the loads at once and expose the memory latency of
-      // every stage; c, d - c, c + d are formed when the stage is generated).  (C_in F) % 4 == 0: every chunk of a stage is valid.
-      auto load_x = [&](int sl, float (&x)[NX]) {
-        if (MODE == 1) {
-          const float* p0 = xp + (size_t)(4 * sl) * istride;
+      auto zf = [&](const float (&y)[2], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+        float v[2][4];
 #pragma unroll
-          for (int c = 0; c < 4; ++c) x[c] = __ldg(p0 + c * istride);
-        } else if (MODE == 2) {
-          const size_t o = (size_t)(2 * sl) * istride;
+        for (int rs = 0; rs < 2; ++rs)
 #pragma unroll
-          for (int il = 0; il < 2; ++il) { x[2 * il] = __ldg(xp + o + il * istride); x[2 * il + 1] = __ldg(xm + o + il * istride); }
-        } else {
-          // chunk c of the stage = K chunk q = 4 sl + c of the segment: input channel q / 3, weight set q % 3
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const size_t o = (size_t)((4 * sl + c) / 3) * istride;
-            x[c] = __ldg(xp + o);
-            x[4 + c] = __ldg(xm + o);
-          }
-        }
+          for (int q = 0; q < 4; ++q) v[rs][q] = u[rs][q] * y[rs];
+        z_frag(v, hi, lo);
       };
-      int sl = (s0 ^ h) & 1;                   // this warp's first stage of the segment
-      float xv[NX];
-#pragma unroll
-      for (int c = 0; c < NX; ++c) xv[c] = 0.f;
-      if (sl < ns) load_x(sl, xv);
+      // (C_in F) % 4 == 0: every chunk of a stage is valid; X is padded to whole edge tiles, so rows past E are readable
 #pragma unroll 1
-      for (; sl < ns; sl += 2) {
-        const int s = s0 + sl;
-        float xn[NX];
+      for (int sl = 0; sl < ns; ++sl, ++s) {
+        if constexpr (MODE == 1) {
+          float y[4][2];
 #pragma unroll
-        for (int c = 0; c < NX; ++c) xn[c] = 0.f;
-        if (sl + 2 < ns) load_x(sl + 2, xn);   // this warp's next stage: prefetched one generation ahead
-        // drain every accumulation block that ended at least AS stages ago (the MMA warp cannot run further ahead anyway)
-        while (flushed < n_blk && s >= next_drain) { drain(); next_drain = min((flushed + 1) * FS, S) - 1 + AS; }
-        const int aslot = s & (AS - 1);
-        mbar_wait(bar_a_empty + 8 * aslot, ((uint32_t)(s >> LOG_AS) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t a0 = tmem_base + t_lane + kZACol + (uint32_t)(aslot * ASLOT);
-        if (MODE == 1 || MODE == 3) {
+          for (int c = 0; c < 4; ++c)
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            uint32_t r[16];
-            float y = xv[c];
-            if (MODE == 3) {
-              const int ty = (sl + c) % 3;                         // weight set (a+b, a, b) <-> y = (c, d - c, c + d)
-              y = (ty == 0) ? xv[c] : (ty == 1) ? (xv[4 + c] - xv[c]) : (xv[c] + xv[4 + c]);
+            for (int rs = 0; rs < 2; ++rs) y[c][rs] = __ldg(xp + (size_t)(4 * sl + c) * istride + 8 * rs);
+          uint64_t b_hi, b_lo;
+          wait_stage(s, b_hi, b_lo);
+          uint32_t hi[4][4], lo[4][4];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) zf(y[c], hi[c], lo[c]);
+          wgmma_fence();
+#pragma unroll
+          for (int c = 0; c < 4; ++c) z_mma3<NR>(D[0], hi[c], lo[c], b_hi + 2 * c, b_lo + 2 * c);
+        } else if constexpr (MODE == 2) {
+          // input channels 2 sl + il; chunk 2 il + f, f in (a, b).  component +m: (a: U x+), (b: -U x-); component -m: (a: U x-), (b: U x+)
+          float yp[2][2], ym[2][2];
+#pragma unroll
+          for (int il = 0; il < 2; ++il)
+#pragma unroll
+            for (int rs = 0; rs < 2; ++rs) {
+              const size_t o = (size_t)(2 * sl + il) * istride + 8 * rs;
+              yp[il][rs] = __ldg(xp + o);
+              ym[il][rs] = __ldg(xm + o);
             }
-            z_outer16(Uh, Ul, y * sxe, r);
-            tmem_st16(a0 + (uint32_t)(c * 16), r);
-          }
-        } else {
+          uint64_t b_hi, b_lo;
+          wait_stage(s, b_hi, b_lo);
+          uint32_t hp[2][4], lp[2][4], hm[2][4], lm[2][4];
 #pragma unroll
           for (int il = 0; il < 2; ++il) {
-            uint32_t rP[16], rM[16], nM[16];
-            z_outer16(Uh, Ul, xv[2 * il] * sxe, rP);
-            z_outer16(Uh, Ul, xv[2 * il + 1] * sxe, rM);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) nM[j] = rM[j] ^ 0x80008000u;
-            // component +m: (f = a: U x+), (f = b: -U x-);   component -m: (f = a: U x-), (f = b: U x+)
-            tmem_st16(a0 + (uint32_t)((2 * il) * 16), rP);
-            tmem_st16(a0 + (uint32_t)((2 * il + 1) * 16), nM);
-            tmem_st16(a0 + (uint32_t)(64 + (2 * il) * 16), rM);
-            tmem_st16(a0 + (uint32_t)(64 + (2 * il + 1) * 16), rP);
+            zf(yp[il], hp[il], lp[il]);
+            zf(ym[il], hm[il], lm[il]);
           }
-        }
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) { if (PAIR && crank != 0) mbar_arrive_remote(bar_a_full + 8 * aslot, 0u); else mbar_arrive(bar_a_full + 8 * aslot); }
+          uint32_t hn[2][4], ln[2][4];         // -U x-
 #pragma unroll
-        for (int c = 0; c < NX; ++c) xv[c] = xn[c];
+          for (int il = 0; il < 2; ++il)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) { hn[il][q] = hm[il][q] ^ 0x80008000u; ln[il][q] = lm[il][q] ^ 0x80008000u; }
+          wgmma_fence();
+#pragma unroll
+          for (int il = 0; il < 2; ++il) {
+            const uint64_t ba_hi = b_hi + 2 * (2 * il), ba_lo = b_lo + 2 * (2 * il);
+            const uint64_t bb_hi = b_hi + 2 * (2 * il + 1), bb_lo = b_lo + 2 * (2 * il + 1);
+            z_mma3<NR>(D[0], hp[il], lp[il], ba_hi, ba_lo);
+            z_mma3<NR>(D[0], hn[il], ln[il], bb_hi, bb_lo);
+            z_mma3<NR>(D[NA - 1], hm[il], lm[il], ba_hi, ba_lo);
+            z_mma3<NR>(D[NA - 1], hp[il], lp[il], bb_hi, bb_lo);
+          }
+        } else {
+          // chunk c of the stage = K chunk q = 4 sl + c of the segment: input channel q / 3, weight set q % 3 <-> y = (c, d - c, c + d)
+          float y[4][2];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const int q = 4 * sl + c;
+            const int ty = q % 3;
+#pragma unroll
+            for (int rs = 0; rs < 2; ++rs) {
+              const size_t o = (size_t)(q / 3) * istride + 8 * rs;
+              const float cp = __ldg(xp + o), dm = __ldg(xm + o);
+              y[c][rs] = (ty == 0) ? cp : (ty == 1) ? (dm - cp) : (cp + dm);
+            }
+          }
+          uint64_t b_hi, b_lo;
+          wait_stage(s, b_hi, b_lo);
+          uint32_t hi[4][4], lo[4][4];
+#pragma unroll
+          for (int c = 0; c < 4; ++c) zf(y[c], hi[c], lo[c]);
+          // the weight set of chunk c is (t0 + c) % 3 with t0 = (4 sl) % 3: one unrolled issue order per t0, so every accumulator
+          // index is a compile-time constant
+          auto issue = [&](auto t0c) {
+            constexpr int T0 = decltype(t0c)::value;
+            wgmma_fence();
+            z_mma3<NR>(D[(T0 + 0) % 3], hi[0], lo[0], b_hi + 0, b_lo + 0);
+            z_mma3<NR>(D[(T0 + 1) % 3], hi[1], lo[1], b_hi + 2, b_lo + 2);
+            z_mma3<NR>(D[(T0 + 2) % 3], hi[2], lo[2], b_hi + 4, b_lo + 4);
+            z_mma3<NR>(D[(T0 + 3) % 3], hi[3], lo[3], b_hi + 6, b_lo + 6);
+          };
+          const int t0 = (4 * sl) % 3;
+          if (t0 == 0) issue(std::integral_constant<int, 0>());
+          else if (t0 == 1) issue(std::integral_constant<int, 1>());
+          else issue(std::integral_constant<int, 2>());
+        }
+        finish_stage(s);
       }
-      s0 += ns;
     }
-    while (flushed < n_blk) drain();
 
-    // out'[e, component plane, channels of this tile]
-    if (active && live) {
-      const float inv = 1.f / sxe;
-      if (MODE == 3) {
+    // out'[e, component plane, channels of this CTA]
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          float* dst = prm.out + (size_t)eg * prm.out_es + prm.comp_off[c] + (size_t)nt * N + h * 64;
+    for (int rs = 0; rs < 2; ++rs) {
+      if (!live[rs]) continue;
+      const float inv = 1.f / sxe[rs];
 #pragma unroll
-          for (int j = 0; j < 64; j += 4)
-            *reinterpret_cast<float4*>(dst + j) = make_float4(acc[c * 64 + j] * inv, acc[c * 64 + j + 1] * inv, acc[c * 64 + j + 2] * inv,
-                                                              acc[c * 64 + j + 3] * inv);
-        }
-      } else {
-        float* dst;
-        if (MODE == 1) dst = prm.out + (size_t)eg * prm.out_es + prm.comp_off[0] + (size_t)nt * N + h * ACC;
-        else dst = prm.out + (size_t)eg * prm.out_es + prm.comp_off[h] + (size_t)nt * N;
+      for (int a = 0; a < NO; ++a) {
+        float* dst = prm.out + (size_t)eg[rs] * prm.out_es + prm.comp_off[a] + (size_t)nt * N + (size_t)hs * NC + kq;
 #pragma unroll
-        for (int j = 0; j < ACC; j += 4)
-          *reinterpret_cast<float4*>(dst + j) = make_float4(acc[j] * inv, acc[j + 1] * inv, acc[j + 2] * inv, acc[j + 3] * inv);
+        for (int g = 0; g < NC / 8; ++g)
+          *reinterpret_cast<float2*>(dst + 8 * g) = make_float2(acc[a][4 * g + 2 * rs] * inv, acc[a][4 * g + 2 * rs + 1] * inv);
       }
     }
-    }   // MODE != 4
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (CSZ > 1) cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kZTmemCols) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kZTmemCols) : "memory");
   }
 }
 
@@ -595,27 +395,17 @@ __global__ void zpack_kernel(const float* __restrict__ Fp, int Kp, int col0, int
   }
 }
 
-template <int MODE, int N, int CSZ, bool PAIR = false>
+template <int MODE, int N, int NC>
 static int launch_z(const ZParams& prm, cudaStream_t s) {
-  constexpr uint32_t kStageBytes = PAIR ? N * 128u : 2u * N * 128u;
+  constexpr uint32_t kStageBytes = 2u * NC * 128u;
   constexpr int WS = (kZWRingBytes / kStageBytes > 8) ? 8 : (int)(kZWRingBytes / kStageBytes);
-  const size_t smem = 1024 + (size_t)WS * kStageBytes + 512;
-  auto kern = zgemm_kernel<MODE, N, CSZ, PAIR>;
+  const size_t smem = 1024 + (size_t)WS * kStageBytes + 256;
+  auto kern = zgemm_kernel<MODE, N, NC>;
   SE3_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int64_t n_mg = (prm.n_mt + CSZ - 1) / CSZ;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(n_mg * prm.n_nt * CSZ));
-  cfg.blockDim = dim3(kZThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CSZ;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  SE3_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, prm));
+  const int64_t grid = (int64_t)prm.n_mt * prm.n_nt * (N / NC);
+  SE3_REQUIRE(grid < 2147483647ll, "se3_zgemm: grid too large");
+  kern<<<(unsigned)grid, kZThreads, smem, s>>>(prm);
+  SE3_LAUNCH_OK();
   return SE3_OK;
 }
 
@@ -685,9 +475,7 @@ extern "C" int se3_linear_tc_fwd(const float* x, const void* w_img, const float*
   prm.n_nt = Eo / 128;
   prm.S = D / 64;
   prm.flush_stages = std::max(1, z_env_int("SE3B200_Z_FLUSH", 8));
-  const int csz = z_env_int("SE3B200_Z_CLUSTER", 2) == 1 ? 1 : 2;
-  cudaStream_t s = as_stream(stream);
-  return csz == 1 ? launch_z<4, 128, 1>(prm, s) : launch_z<4, 128, 2>(prm, s);
+  return launch_z<4, 128, 128>(prm, as_stream(stream));
 }
 
 extern "C" int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img, const float* sx, int64_t E, int Co, int mode,
@@ -728,26 +516,12 @@ extern "C" int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img,
   prm.n_mt = (int)ceil_div(E, SE3_TILE_E);
   prm.n_nt = Co / N;
   prm.S = S;
-  // default drain period: 96 accumulating tcgen05.mma per accumulator (8 stages of 12; mode 3 spreads its stages over three
+  // default drain period: 96 accumulating K = 16 MMAs per accumulator (8 stages of 12; mode 3 spreads its stages over three
   // accumulators): rel. error 4e-6 against float64 for all-positive operands at K = 65536 (2.5e-4 if never drained)
   prm.flush_stages = std::max(1, flush_stages > 0 ? flush_stages
                                                      : z_env_int("SE3B200_Z_FLUSH", mode == 3 ? 24 : 8) * std::max(1, z_env_int("SE3B200_Z_FLUSH_MULT", 1)));
-  const int csz_env = z_env_int("SE3B200_Z_CLUSTER", 2);
-  const int csz = csz_env == 1 ? 1 : (csz_env == 4 && prm.n_mt % 4 == 0 && mode != 2) ? 4 : 2;
-  // cta_group::2 pair mode vs 2-CTA multicast of W.  SE3B200_Z_PAIR: bit 0 = MODE 1, bit 1 = MODE 3; default 0 (off).
-  // Measured (cfg2 depth-1 slice, same box, profiles/r02_pair_mode.md): in pair mode MODE 1 (N = 256, four A stages) issues 1.70
-  // instead of 1.50 PFLOP/s -- half the weight traffic per SM lets the SM clock rise from 1.45 to 1.86 GHz -- but MODE 3 (two
-  // 768-cycle A stages) cannot hide the cross-SM hand-off (remote mbarrier arrive + multicast commit per stage): 1.03 instead of
-  // 1.50 PFLOP/s; with MODE 1 alone in pair mode the power budget saved there is spent by MODE 3 and the step time is unchanged.
-  const int pair_bits = csz == 2 ? z_env_int("SE3B200_Z_PAIR", 0) : 0;
-  const bool pair = (pair_bits & (mode == 3 ? 2 : 1)) != 0;
   cudaStream_t s = as_stream(stream);
-  if (csz == 4) {                            // 4-CTA multicast of W (experiment: a quarter of the L2 reads per SM)
-    if (mode == 3) return launch_z<3, 128, 4>(prm, s);
-    return N == 256 ? launch_z<1, 256, 4>(prm, s) : launch_z<1, 128, 4>(prm, s);
-  }
-  if (mode == 3) return csz == 1 ? launch_z<3, 128, 1>(prm, s) : pair ? launch_z<3, 128, 2, true>(prm, s) : launch_z<3, 128, 2>(prm, s);
-  if (mode == 2) return csz == 1 ? launch_z<2, 128, 1>(prm, s) : launch_z<2, 128, 2>(prm, s);
-  if (N == 256) return csz == 1 ? launch_z<1, 256, 1>(prm, s) : pair ? launch_z<1, 256, 2, true>(prm, s) : launch_z<1, 256, 2>(prm, s);
-  return csz == 1 ? launch_z<1, 128, 1>(prm, s) : pair ? launch_z<1, 128, 2, true>(prm, s) : launch_z<1, 128, 2>(prm, s);
+  if (mode == 3) return launch_z<3, 128, 64>(prm, s);
+  if (mode == 2) return launch_z<2, 128, 64>(prm, s);
+  return N == 256 ? launch_z<1, 256, 128>(prm, s) : launch_z<1, 128, 128>(prm, s);
 }

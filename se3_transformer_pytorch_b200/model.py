@@ -3,7 +3,7 @@
 Same constructor, forward signature, assertions and state_dict key/shape layout as
 lucidrains/se3-transformer-pytorch v0.9.0 (se3_transformer_pytorch.py:936-1375; SURVEY.md Appendix A.6), so
 `ours.load_state_dict(reference.state_dict())` works.  The hot path -- neighbour graph, spherical-harmonic / CG basis,
-radial trunk, pairwise tensor product (tcgen05), pooling, attention -- runs in the hand-written sm_100a kernels of
+radial trunk, pairwise tensor product (wgmma), pooling, attention -- runs in the hand-written sm_90a kernels of
 libse3b200.so through `ops`; the cheap glue around it (embeddings, LinearSE3 GEMMs, NormSE3, residuals) stays torch.
 
 Forward only: everything runs under torch.no_grad().  CUDA only: there is no CPU fallback.
@@ -247,7 +247,7 @@ class ConvSE3(nn.Module):
         return self._packed
 
     def tc_eligible(self, di, do):
-        """The tcgen05 kernels take this pair: sm_100, C_out % 32 == 0, degree_out <= 3 and operands inside the fp16 range
+        """The tensor-core kernels take this pair: sm_90, C_out % 32 == 0, degree_out <= 3 and operands inside the fp16 range
         of the hi/lo split (|g| <= sqrt(127) max|ln.w| + max|ln.b| after LayerNorm + GELU)."""
         pk = self.packed()
         if (di, do) not in pk['tc_ok']:
@@ -1010,7 +1010,7 @@ def masked_mean_nodes(t, mask):
 
 
 class SE3Transformer(nn.Module):
-    """Drop-in for se3_transformer_pytorch.SE3Transformer (reference S:936-1375), inference on B200.
+    """Drop-in for se3_transformer_pytorch.SE3Transformer (reference S:936-1375), inference on H100.
 
     Not carried over (raise NotImplementedError): reversible, use_egnn -- they are outside the hot path named by BASELINE.json
     (SURVEY.md section 2, "OUT OF SCOPE")."""
@@ -1027,7 +1027,7 @@ class SE3Transformer(nn.Module):
         super().__init__()
         for flag, name in ((reversible, 'reversible'), (use_egnn, 'use_egnn')):
             if flag:
-                raise NotImplementedError(f'{name}=True is outside the B200 hot path of this package')
+                raise NotImplementedError(f'{name}=True is outside the H100 hot path of this package')
         if differentiable_coors:
             raise NotImplementedError('differentiable_coors=True needs the backward pass; this package is forward only (SURVEY.md 8f row 4)')
         dim_in = default(dim_in, dim)
@@ -1171,7 +1171,7 @@ class SE3Transformer(nn.Module):
         b, n, d = feats['0'].shape[:3]
         device = feats['0'].device
         if not coors.is_cuda:
-            raise RuntimeError('se3_transformer_pytorch_b200 runs on CUDA (sm_100a) only; move the model and inputs to the GPU')
+            raise RuntimeError('se3_transformer_pytorch_b200 runs on CUDA (sm_90a) only; move the model and inputs to the GPU')
         assert d == self.dim_in[0], f'feature dimension {d} must be equal to dimension given at init {self.dim_in[0]}'
         assert set(map(int, feats.keys())) == set(range(self.input_degrees)), f'input must have {self.input_degrees} degree'
         feats = {k: v.float().contiguous() for k, v in feats.items()}

@@ -1,7 +1,7 @@
 """ctypes binding of libse3b200.so (C ABI in include/se3b200.h) for torch CUDA tensors.
 
 PyTorch is plumbing here: it owns device memory and the current stream; every op below hands raw device pointers
-and the stream handle to the hand-written sm_100a kernels.  There is NO CPU fallback: calling an op with a
+and the stream handle to the hand-written sm_90a kernels.  There is NO CPU fallback: calling an op with a
 non-CUDA tensor, or without the compiled library, raises.
 """
 import ctypes
@@ -36,7 +36,6 @@ _SIGNATURES = {
     'se3_pack_lowrank': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_pairwise_lr_fwd': (c_int, [c_void_p] * 3 + [c_int64] + [c_int] * 6 + [c_void_p, c_void_p]),
     'se3_pairwise_lr_strided_fwd': (c_int, [c_void_p] * 3 + [c_int64] + [c_int] * 6 + [c_void_p, c_int64, c_int, c_void_p, c_void_p]),
-    'se3_pairwise_lr_trace': (c_int, [c_void_p] * 3 + [c_int64] + [c_int] * 6 + [c_void_p, c_void_p, c_void_p]),
     'se3_fold_basis_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_fold_basis_cm_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_rotate_back_fwd': (c_int, [c_void_p] * 5 + [c_int64, c_int, c_int, c_void_p, c_void_p]),
@@ -112,7 +111,7 @@ class _timed:
 def _require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError('se3_transformer_pytorch_b200 runs on CUDA (sm_100a) only: got a tensor on %s; '
+            raise RuntimeError('se3_transformer_pytorch_b200 runs on CUDA (sm_90a) only: got a tensor on %s; '
                                'there is no CPU path' % t.device)
 
 
@@ -589,7 +588,7 @@ def linear_supported(D, Eo, device):
     """Shapes the tensor-core LinearSE3 kernel takes."""
     if os.environ.get('SE3B200_NO_LINEAR_TC') or os.environ.get('SE3B200_FORCE_SIMT'):
         return False
-    return D % 64 == 0 and Eo % 128 == 0 and torch.cuda.get_device_capability(device)[0] == 10
+    return D % 64 == 0 and Eo % 128 == 0 and torch.cuda.get_device_capability(device) == (9, 0)
 
 
 def linear_image(W):
@@ -679,8 +678,8 @@ def zgemm(segs, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off, flush_st
 
 # max-abs residual of the radial basis relative to max|G|.  The fp32 trunk itself carries ~6e-7..1e-6 of rounding noise
 # against float64, so 1e-6 keeps the truncation below what fp32 can resolve; at the headline width (depth-2 slice of cfg2)
-# the output differs from the fp32 SIMT path by 1.6e-5 with 1e-6 and by 1.5e-5 with 2e-7 or with the direct K = 128 kernel
-# (tools/lr_tol_check.py).  With 1e-6, 96 % of the cfg2 pairs need rank <= 15 (K = 16) instead of 26 % with 2e-7.
+# the output differs from the fp32 SIMT path by 1.6e-5 with 1e-6 and by 1.5e-5 with 2e-7 or with the direct K = 128
+# kernel.  With 1e-6, 96 % of the cfg2 pairs need rank <= 15 (K = 16) instead of 26 % with 2e-7.
 LOWRANK_TOL = 1e-6
 
 
@@ -716,12 +715,12 @@ def lowrank_enabled(E):
 
 
 def tc_supported(device, Co, P):
-    """The tcgen05 kernel needs sm_100 and Co % 32 == 0, degree_out <= 3."""
+    """The wgmma kernel needs sm_90 and Co % 32 == 0, degree_out <= 3."""
     if os.environ.get('SE3B200_FORCE_SIMT'):
         return False
     if Co % TILE_O != 0 or P > 7:
         return False
-    return torch.cuda.get_device_capability(device)[0] == 10
+    return torch.cuda.get_device_capability(device) == (9, 0)
 
 
 def pool(x, mask):

@@ -1,12 +1,13 @@
-"""Golden-vector generator.  DEV-CONTAINER ONLY: imports the real reference from
-/root/reference (read-only) and writes small fixtures that travel with the repo.
+"""Golden-vector generator.  Needs a checkout of the real reference (lucidrains/se3-transformer-pytorch) on the Python path
+and writes small fixtures that travel with the repo; the tests themselves never import the reference.
 
-    PYTHONPATH=/root/reference CACHE_PATH=/tmp/se3_cache python tests/golden/gen_golden.py
+    PYTHONPATH=<reference checkout> CACHE_PATH=/tmp/se3_cache python tests/golden/gen_golden.py
 
 Outputs
   se3_transformer_pytorch_b200/data/qj_tables.npz   Q_J change-of-basis tables (reference basis.py:123-138)
   tests/golden/sh_basis.npz                         Y_J + get_basis on fixed vectors (basis.py:140-205)
-  tests/golden/model_<case>.npz                     whole-model inputs/outputs + captured intermediates
+  tests/golden/model_<case>.npz                     whole-model inputs/outputs + captured intermediates (largest arrays
+                                                    in model_<case>.part<i>.npz, so that every file stays under 1 MB)
   tests/golden/state_keys.json                      state_dict key/shape lists (SURVEY.md A.6)
 
 Weights are never stored: both sides fill state_dict() with tests/golden/detfill.py.
@@ -18,7 +19,6 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, HERE)
-sys.path.insert(0, '/root/reference')
 os.environ.setdefault('CACHE_PATH', '/tmp/se3_cache')
 
 from detfill import fill_state_dict, det_inputs, det_uniform  # noqa: E402
@@ -270,10 +270,33 @@ def run_case(case):
     out['config'] = np.array(json.dumps(dict(ctor={k: (list(v) if isinstance(v, tuple) else v) for k, v in case['ctor'].items()},
                                              fwd=case.get('fwd', {}), b=case['b'], n=case['n'])))
     path = os.path.join(HERE, f'model_{name}.npz')
-    np.savez_compressed(path, **out)
+    write_split(path, out)
     keys = {k: list(v.shape) for k, v in model.state_dict().items()}
     print('wrote', path, 'params', sum(int(np.prod(s)) for s in keys.values()), 'size', os.path.getsize(path))
     return keys
+
+
+def write_split(path, arrays, limit=900_000):
+    """np.savez_compressed(path, **arrays), moving the largest arrays one by one into path.part<i>.npz files while a file
+    would exceed `limit` bytes (tests/helpers.py:load_case merges them back)."""
+    import io
+    for old in [f for f in os.listdir(HERE) if f.startswith(os.path.basename(path)[:-4] + '.part')]:
+        os.remove(os.path.join(HERE, old))
+    main = dict(arrays)
+    size = lambda d: (lambda b: (np.savez_compressed(b, **d), b.tell())[1])(io.BytesIO())
+    parts = []
+    for k in sorted(main, key=lambda k: -main[k].nbytes):
+        if size(main) <= limit:
+            break
+        if k == 'config':
+            continue
+        if parts and size({**parts[-1], k: main[k]}) <= limit:
+            parts[-1][k] = main.pop(k)
+        else:
+            parts.append({k: main.pop(k)})
+    np.savez_compressed(path, **main)
+    for i, part in enumerate(parts):
+        np.savez_compressed(f'{path[:-4]}.part{i + 2}.npz', **part)
 
 
 def gen_equivariance_inputs():

@@ -19,6 +19,9 @@ Z_CASES = ['z128', 'z256_deg4']
 
 def load_case(name):
     z = dict(np.load(os.path.join(GOLDEN, f'model_{name}.npz')))
+    # the largest fixtures are split into model_<name>.part<i>.npz files (each stored file stays under 1 MB)
+    for part in sorted(f for f in os.listdir(GOLDEN) if f.startswith(f'model_{name}.part')):
+        z.update(np.load(os.path.join(GOLDEN, part)))
     cfg = json.loads(str(z.pop('config')))
     ctor = cfg['ctor']
     if isinstance(ctor.get('dim_in'), list):

@@ -93,7 +93,7 @@ def test_production_path_matches_oracle_at_headline_width(k_nbr, n):
     """cfg2 shape (N = 1024, k = 16: E = 16384 per cloud) and cfg5 shape (N = 2048, k = 32: E = 65536), one cloud, depth 1."""
     from se3_transformer_pytorch_b200 import SE3Transformer, ops
     if not ops.tc_supported(DEV, 512, 7):
-        pytest.skip('needs sm_100')
+        pytest.skip('needs sm_90')
     nd, dim, heads, dim_head = 4, 512, 8, 64
     torch.manual_seed(0)
     with torch.device(DEV):
@@ -125,7 +125,7 @@ def test_production_path_matches_simt_whole_model():
     """Whole model at cfg2 widths, depth 1, E = 16384: production dispatch vs the fp32 SIMT kernels on the same weights."""
     from se3_transformer_pytorch_b200 import SE3Transformer, ops
     if not ops.tc_supported(DEV, 512, 7):
-        pytest.skip('needs sm_100')
+        pytest.skip('needs sm_90')
     torch.manual_seed(1)
     with torch.device(DEV):
         model = SE3Transformer(dim=512, heads=8, dim_head=64, depth=1, num_degrees=4, output_degrees=2, num_neighbors=16).eval()
@@ -177,7 +177,7 @@ def test_plan_guard_bounds_the_output_error(radial, monkeypatch):
     import json
     from se3_transformer_pytorch_b200 import SE3Transformer, ops, model as M
     if not ops.tc_supported(DEV, 128, 1):
-        pytest.skip('needs sm_100')
+        pytest.skip('needs sm_90')
     if radial == 'mlp':
         monkeypatch.setenv('SE3B200_NO_UTABLE', '1')
     ctor = dict(dim=128, heads=2, dim_head=64, depth=1, num_degrees=3, output_degrees=2, num_neighbors=8)

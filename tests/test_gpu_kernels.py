@@ -183,7 +183,7 @@ def test_pairwise_tc_matches_fp64(di, do, Ci, Co, n, k):
     """tcgen05 kernel (3-pass bf16 split) vs float64 numpy: 2e-5 relative; also the raw R tile of step 0."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, Co, 2 * do + 1):
-        pytest.skip('tensor-core path needs sm_100')
+        pytest.skip('tensor-core path needs sm_90')
     rng = np.random.default_rng(7)
     pr = _pair_problem(rng, 1, n, k, Ci, Co, di, do)
     E, P, F = pr['E'], pr['P'], pr['F']
@@ -212,7 +212,7 @@ def test_pairwise_tc_cluster_sizes(csz, monkeypatch):
     """W-multicast cluster sizes 1/2/4 (incl. a padded last cluster: 5 edge tiles) give the same result."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, 64, 5):
-        pytest.skip('tensor-core path needs sm_100')
+        pytest.skip('tensor-core path needs sm_90')
     monkeypatch.setenv('SE3B200_TC_CLUSTER', str(csz))
     rng = np.random.default_rng(9)
     di, do, Ci, Co = 2, 2, 12, 64
@@ -229,7 +229,7 @@ def test_pairwise_lowrank_matches_fp64(r, P, di, do):
     """Low-rank radial kernel: G = U V^T exactly of rank r; result vs float64 of the original (K = 128) contraction."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, 64, P):
-        pytest.skip('tensor-core path needs sm_100')
+        pytest.skip('tensor-core path needs sm_90')
     rng = np.random.default_rng(11)
     Ci, Co = 10, 64
     pr = _pair_problem(rng, 1, 30, 9, Ci, Co, di, do)             # E = 270 -> 3 edge tiles (one padding CTA in a 2-cluster)
@@ -259,7 +259,7 @@ def test_input_side_contraction_matches_fp64(r, di, do):
     from se3_transformer_pytorch_b200 import ops
     P, Q = 2 * do + 1, 2 * di + 1
     if not ops.tc_supported(DEV, 64, P):
-        pytest.skip('tensor-core path needs sm_100')
+        pytest.skip('tensor-core path needs sm_90')
     rng = np.random.default_rng(17)
     Ci, Co = 12, 64
     pr = _pair_problem(rng, 1, 30, 9, Ci, Co, di, do)
@@ -315,7 +315,7 @@ def test_pairwise_tc_headline_width_matches_simt():
     """BASELINE cfg2 widths (C_in = C_out = 512, degree 3 -> 3) on a small edge set: tensor-core vs SIMT fp32."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, 512, 7):
-        pytest.skip('tensor-core path needs sm_100')
+        pytest.skip('tensor-core path needs sm_90')
     torch.manual_seed(0)
     b, n, k, C, di, do = 1, 24, 8, 512, 3, 3
     E, P, Q, F = b * n * k, 7, 7, 7

@@ -86,7 +86,7 @@ def test_zgemm_matches_fp64(mode, Co, E, segs, pair, monkeypatch):
     weights; an option, off by default -- see se3_zgemm_fwd)."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, Co, 1):
-        pytest.skip('needs sm_100')
+        pytest.skip('needs sm_90')
     if pair and mode == 2:
         pytest.skip('pair mode exists for modes 1 and 3')
     monkeypatch.setenv('SE3B200_Z_PAIR', str(pair))
@@ -101,7 +101,7 @@ def test_zgemm_is_scale_invariant(x_scale):
     """The per-edge power-of-two scale keeps the fp16 operands in range whatever the magnitude of the features."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, 128, 1):
-        pytest.skip('needs sm_100')
+        pytest.skip('needs sm_90')
     for mode in (2, 3):
         out, ref = _run_zgemm(mode, 128, 200, [(8, 3, 2, 0, 16)], x_scale=x_scale)
         assert rel_err(out.cpu().numpy(), ref.cpu().numpy()) < 6e-6
@@ -114,7 +114,7 @@ def test_zgemm_headline_width_long_k(mode):
     result within 1e-5 of float64 (the error without it is recorded next to it)."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, 512, 1):
-        pytest.skip('needs sm_100')
+        pytest.skip('needs sm_90')
     segs = [(512, 2 * l + 1, l + (1 if mode >= 2 and l else 0), l - (1 if mode >= 2 and l else 0), 16) for l in ((0, 1, 2, 3) if mode == 1 else (1, 2, 3))]
     out, ref = _run_zgemm(mode, 512, 512, segs, flush=0, positive=True)
     err = rel_err(out.cpu().numpy(), ref.cpu().numpy())
@@ -291,7 +291,7 @@ def test_linear_tc_matches_fp64(D, Eo, M, nodes, with_res):
     fused residual and with features of very different magnitude per node (the per-node power-of-two scale)."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.linear_supported(D, Eo, DEV):
-        pytest.skip('needs sm_100')
+        pytest.skip('needs sm_90')
     g = torch.Generator().manual_seed(D + M)
     x = torch.randn(1, nodes, D, M, generator=g)
     x = x * torch.logspace(-6, 4, nodes).view(1, nodes, 1, 1)          # per-node magnitudes 1e-6 .. 1e4
