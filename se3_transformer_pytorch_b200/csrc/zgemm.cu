@@ -24,8 +24,9 @@
 // 384 threads: warp 0 streams the weight image (TMA bulk copies into an mbarrier ring); warpgroups 1 and 2 own 64 edge rows
 // each, generate Z for their rows, issue m64 x NC x 16 wgmma with A from registers and B from shared memory, and keep the
 // fp32 partial sums: tensor-core accumulation truncates, so every `flush_stages` stages the accumulators are added into
-// registers with round-to-nearest adds and restarted.  The two warpgroups interleave, so one's MMAs overlap the other's
-// generation.
+// registers with round-to-nearest adds and restarted.  MODE 1 / 3 commit one wgmma group per K chunk and generate the next chunk
+// while the previous chunks' MMAs are in flight, with X loaded into registers a stage (MODE 1) or a 3-stage period (MODE 3)
+// ahead; MODE 2 / 4 wait for their MMAs every stage.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include <algorithm>
@@ -37,6 +38,19 @@ namespace se3 {
 constexpr int kZThreads = 384;
 constexpr int kZMaxSeg = 16;
 constexpr uint32_t kZWRingBytes = 196608;     // shared memory for the weight ring
+
+template <int V>
+using ic = std::integral_constant<int, V>;
+
+// f(ic<0>()), ..., f(ic<N - 1>()): fully unrolled, the index a compile-time constant in every call
+template <class F, int... I>
+__device__ __forceinline__ void static_for_seq(F&& f, std::integer_sequence<int, I...>) {
+  (f(ic<I>()), ...);
+}
+template <int N, class F>
+__device__ __forceinline__ void static_for(F&& f) {
+  static_for_seq(f, std::make_integer_sequence<int, N>());
+}
 
 struct ZSeg {
   const float* U;      // [E, 64] fp32 (this sub-segment reads columns 0..15 from the pointer given)
@@ -65,13 +79,14 @@ __device__ __forceinline__ void z_frag(const float (&v)[2][4], uint32_t (&hi)[4]
 }
 
 template <int NR>
-__device__ __forceinline__ void z_mma3(float (&d)[NR], const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint64_t b_hi, uint64_t b_lo) {
+__device__ __forceinline__ void z_mma3(float (&d)[NR], const uint32_t (&hi)[4], const uint32_t (&lo)[4], uint64_t b_hi, uint64_t b_lo,
+                                       uint32_t scale_d = 1) {
   if constexpr (NR == 64) {
-    wgmma_rs_n128(d, hi, b_hi);
+    wgmma_rs_n128(d, hi, b_hi, scale_d);
     wgmma_rs_n128(d, lo, b_hi);
     wgmma_rs_n128(d, hi, b_lo);
   } else {
-    wgmma_rs_n64(d, hi, b_hi);
+    wgmma_rs_n64(d, hi, b_hi, scale_d);
     wgmma_rs_n64(d, lo, b_hi);
     wgmma_rs_n64(d, hi, b_lo);
   }
@@ -152,27 +167,72 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
 #pragma unroll
     for (int j = 0; j < NR; ++j) acc[a][j] = 0.f;
   int blk_start = 0;
+  // MODE 1 / 3 restart a drained accumulator with the first MMA that writes it (scale-d = 0) instead of zeroing its registers,
+  // so D is written only by wgmma (bit a: accumulator a is drained).  Every stage writes every accumulator, so each block of
+  // flush_stages stages restarts all of them before the next drain.
+  int fresh = 0;
 
-  // after stage s: hand the weight slot back, drain the accumulators at the end of a block
+  auto release = [&](int s) {                  // every MMA that read the weight slot of stage s has retired
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_w_empty + 8 * (s % WS));
+  };
+  // the accumulators are added into the fp32 partial sums at the end of each block of flush_stages stages, and after the last
+  auto drain_after = [&](int s) { return s + 1 == S || s + 1 - blk_start == FS; };
+  auto drain = [&](int s) {
+#pragma unroll
+    for (int j = 0; j < NR; ++j) {
+      if (MODE == 3) {
+        acc[0][j] += D[0][j] - D[NA - 1][j];
+        acc[1][j] += D[0][j] + D[NA > 1 ? 1 : 0][j];
+      } else {
+#pragma unroll
+        for (int a = 0; a < NA; ++a) acc[a][j] += D[a][j];
+      }
+      if (MODE == 2 || MODE == 4)
+#pragma unroll
+        for (int a = 0; a < NA; ++a) D[a][j] = 0.f;
+    }
+    fresh = (1 << NA) - 1;
+    blk_start = s + 1;
+  };
+  // MODE 2 / 4: the MMAs of stage s retire before the next stage is generated
   auto finish_stage = [&](int s) {
     wgmma_commit();
     wgmma_wait0();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_w_empty + 8 * (s % WS));
-    if (s + 1 == S || s + 1 - blk_start == FS) {
+    release(s);
+    if (drain_after(s)) drain(s);
+  };
+
+  // MODE 1 / 3: one commit group per K chunk, so the MMAs of the last ZR - 1 chunks stay in flight while the next chunk's A
+  // fragments are generated
+  constexpr int ZR = (MODE == 3) ? 2 : 4;
+  float u[2][4];                               // U[e, kq, kq+1, kq+8, kq+9] * sx[e] of rows r0, r0 + 8 (current segment)
+  auto zf = [&](const float (&y)[2], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
+    float v[2][4];
 #pragma unroll
-      for (int j = 0; j < NR; ++j) {
-        if (MODE == 3) {
-          acc[0][j] += D[0][j] - D[NA - 1][j];
-          acc[1][j] += D[0][j] + D[NA > 1 ? 1 : 0][j];
-        } else {
+    for (int rs = 0; rs < 2; ++rs)
 #pragma unroll
-          for (int a = 0; a < NA; ++a) acc[a][j] += D[a][j];
-        }
-#pragma unroll
-        for (int a = 0; a < NA; ++a) D[a][j] = 0.f;
-      }
-      blk_start = s + 1;
+      for (int q = 0; q < 4; ++q) v[rs][q] = u[rs][q] * y[rs];
+    z_frag(v, hi, lo);
+  };
+  // chunk C of stage s into accumulator A.  The wait retires chunk k - ZR, whose A fragment registers the new chunk reuses; at
+  // C == ZR - 1 that is the last chunk of stage s - 1, so its weight slot goes back.
+  auto chunk_mma = [&](auto cc, auto ac, int s, const float (&y)[2], uint64_t b_hi, uint64_t b_lo) {
+    constexpr int C = decltype(cc)::value, A = decltype(ac)::value;
+    wgmma_wait<ZR - 1>();
+    if (C == ZR - 1 && s != blk_start) release(s - 1);     // stage s - 1 was not drained: its slot is still held
+    uint32_t hi[4], lo[4];
+    zf(y, hi, lo);
+    wgmma_fence();
+    z_mma3<NR>(D[A], hi, lo, b_hi + 2 * C, b_lo + 2 * C, ((fresh >> A) & 1) ^ 1);
+    fresh &= ~(1 << A);
+    wgmma_commit();
+  };
+  auto end_stage = [&](int s) {
+    if (drain_after(s)) {
+      wgmma_wait0();
+      release(s);
+      drain(s);
     }
   };
   auto wait_stage = [&](int s, uint64_t& b_hi, uint64_t& b_lo) {
@@ -236,7 +296,8 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
         }
     }
   } else {
-    // ---- MODE 1 / 2 / 3
+    // ---- MODE 1 / 2 / 3.  (C_in F) % 4 == 0: every chunk of a stage is valid; X is padded to whole edge tiles, so rows past E
+    // are readable
     int s = 0;                                 // global stage index
     for (int sg = 0; sg < prm.n_seg; ++sg) {
       const ZSeg& z = prm.seg[sg];
@@ -244,39 +305,36 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
       const size_t istride = (size_t)z.ncomp * 128;                     // floats between consecutive input channels of X
       const float* xp = z.X + ((size_t)mt * z.Ci * z.ncomp + z.cplus) * 128 + r0;
       const float* xm = z.X + ((size_t)mt * z.Ci * z.ncomp + z.cminus) * 128 + r0;
-      float u[2][4];                           // U[e, kq, kq+1, kq+8, kq+9] * sx[e] of rows r0, r0 + 8
 #pragma unroll
       for (int rs = 0; rs < 2; ++rs) {
         const float* urow = z.U + (size_t)(live[rs] ? eg[rs] : 0) * 64;
 #pragma unroll
         for (int q = 0; q < 4; ++q) u[rs][q] = live[rs] ? __ldg(urow + kq + (q & 1) + 8 * (q >> 1)) * sxe[rs] : 0.f;
       }
-      auto zf = [&](const float (&y)[2], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
-        float v[2][4];
+      if constexpr (MODE == 1) {
+        // chunk c of stage sl = input channel 4 sl + c; its rows are loaded one stage ahead, as soon as the chunk is generated
+        float y[4][2];
 #pragma unroll
-        for (int rs = 0; rs < 2; ++rs)
+        for (int c = 0; c < 4; ++c)
 #pragma unroll
-          for (int q = 0; q < 4; ++q) v[rs][q] = u[rs][q] * y[rs];
-        z_frag(v, hi, lo);
-      };
-      // (C_in F) % 4 == 0: every chunk of a stage is valid; X is padded to whole edge tiles, so rows past E are readable
+          for (int rs = 0; rs < 2; ++rs) y[c][rs] = __ldg(xp + c * istride + 8 * rs);
 #pragma unroll 1
-      for (int sl = 0; sl < ns; ++sl, ++s) {
-        if constexpr (MODE == 1) {
-          float y[4][2];
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-#pragma unroll
-            for (int rs = 0; rs < 2; ++rs) y[c][rs] = __ldg(xp + (size_t)(4 * sl + c) * istride + 8 * rs);
+        for (int sl = 0; sl < ns; ++sl, ++s) {
+          const float* xn = (sl + 1 < ns) ? xp + 4 * istride : xp;    // the last stage reloads its own rows, never past the tile
           uint64_t b_hi, b_lo;
           wait_stage(s, b_hi, b_lo);
-          uint32_t hi[4][4], lo[4][4];
+          static_for<4>([&](auto cc) {
+            constexpr int C = decltype(cc)::value;
+            chunk_mma(cc, ic<0>(), s, y[C], b_hi, b_lo);
 #pragma unroll
-          for (int c = 0; c < 4; ++c) zf(y[c], hi[c], lo[c]);
-          wgmma_fence();
-#pragma unroll
-          for (int c = 0; c < 4; ++c) z_mma3<NR>(D[0], hi[c], lo[c], b_hi + 2 * c, b_lo + 2 * c);
-        } else if constexpr (MODE == 2) {
+            for (int rs = 0; rs < 2; ++rs) y[C][rs] = __ldg(xn + C * istride + 8 * rs);
+          });
+          end_stage(s);
+          xp = xn;
+        }
+      } else if constexpr (MODE == 2) {
+#pragma unroll 1
+        for (int sl = 0; sl < ns; ++sl, ++s) {
           // input channels 2 sl + il; chunk 2 il + f, f in (a, b).  component +m: (a: U x+), (b: -U x-); component -m: (a: U x-), (b: U x+)
           float yp[2][2], ym[2][2];
 #pragma unroll
@@ -310,41 +368,51 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
             z_mma3<NR>(D[NA - 1], hm[il], lm[il], ba_hi, ba_lo);
             z_mma3<NR>(D[NA - 1], hp[il], lp[il], bb_hi, bb_lo);
           }
-        } else {
-          // chunk c of the stage = K chunk q = 4 sl + c of the segment: input channel q / 3, weight set q % 3 <-> y = (c, d - c, c + d)
-          float y[4][2];
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const int q = 4 * sl + c;
-            const int ty = q % 3;
-#pragma unroll
-            for (int rs = 0; rs < 2; ++rs) {
-              const size_t o = (size_t)(q / 3) * istride + 8 * rs;
-              const float cp = __ldg(xp + o), dm = __ldg(xm + o);
-              y[c][rs] = (ty == 0) ? cp : (ty == 1) ? (dm - cp) : (cp + dm);
-            }
-          }
-          uint64_t b_hi, b_lo;
-          wait_stage(s, b_hi, b_lo);
-          uint32_t hi[4][4], lo[4][4];
-#pragma unroll
-          for (int c = 0; c < 4; ++c) zf(y[c], hi[c], lo[c]);
-          // the weight set of chunk c is (t0 + c) % 3 with t0 = (4 sl) % 3: one unrolled issue order per t0, so every accumulator
-          // index is a compile-time constant
-          auto issue = [&](auto t0c) {
-            constexpr int T0 = decltype(t0c)::value;
-            wgmma_fence();
-            z_mma3<NR>(D[(T0 + 0) % 3], hi[0], lo[0], b_hi + 0, b_lo + 0);
-            z_mma3<NR>(D[(T0 + 1) % 3], hi[1], lo[1], b_hi + 2, b_lo + 2);
-            z_mma3<NR>(D[(T0 + 2) % 3], hi[2], lo[2], b_hi + 4, b_lo + 4);
-            z_mma3<NR>(D[(T0 + 3) % 3], hi[3], lo[3], b_hi + 6, b_lo + 6);
-          };
-          const int t0 = (4 * sl) % 3;
-          if (t0 == 0) issue(std::integral_constant<int, 0>());
-          else if (t0 == 1) issue(std::integral_constant<int, 1>());
-          else issue(std::integral_constant<int, 2>());
+          finish_stage(s);
         }
-        finish_stage(s);
+      } else {
+        // K chunk q = 4 sl + c of the segment: input channel q / 3, weight set q % 3 of (a+b, a, b) <-> y = (c, d - c, c + d).  The
+        // map repeats every 3 stages (12 chunks, 4 input channels) and ns = 3 C_in / 4, so the loop runs over whole periods with
+        // every channel offset and accumulator index known at compile time.  Each (channel, +-m component, row) value is loaded
+        // once per period, one period ahead: channel j of the next period as soon as the last chunk of channel j is generated.
+        const int dmo = (z.cminus - z.cplus) * 128;                   // from x'(+m) to x'(-m) of the same channel
+        float x[4][2][2];                      // [channel of the period][c = x'(+m), d = x'(-m)][row]
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+          for (int rs = 0; rs < 2; ++rs) {
+            x[j][0][rs] = __ldg(xp + j * istride + 8 * rs);
+            x[j][1][rs] = __ldg(xp + dmo + j * istride + 8 * rs);
+          }
+        const int np = ns / 3;
+#pragma unroll 1
+        for (int p = 0; p < np; ++p) {
+          const size_t adv = (p + 1 < np) ? 4 * istride : 0;          // the last period reloads its own rows, never past the tile
+          static_for<3>([&](auto tc) {
+            uint64_t b_hi, b_lo;
+            wait_stage(s, b_hi, b_lo);
+            static_for<4>([&](auto cc) {
+              constexpr int Q = 4 * decltype(tc)::value + decltype(cc)::value, J = Q / 3, T = Q % 3;
+              float y[2];
+#pragma unroll
+              for (int rs = 0; rs < 2; ++rs) {
+                const float cp = x[J][0][rs], dm = x[J][1][rs];
+                y[rs] = (T == 0) ? cp : (T == 1) ? (dm - cp) : (cp + dm);
+              }
+              chunk_mma(cc, ic<T>(), s, y, b_hi, b_lo);
+              if constexpr (T == 2) {
+#pragma unroll
+                for (int rs = 0; rs < 2; ++rs) {
+                  x[J][0][rs] = __ldg(xp + adv + J * istride + 8 * rs);
+                  x[J][1][rs] = __ldg(xp + adv + dmo + J * istride + 8 * rs);
+                }
+              }
+            });
+            end_stage(s);
+            ++s;
+          });
+          xp += adv;
+        }
       }
     }
 
