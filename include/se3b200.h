@@ -5,6 +5,7 @@
  * path binds at the three tensor-only seams of the reference (SURVEY.md section 8b):
  *
  *   neighbour builder inside SE3Transformer.forward   se3_transformer_pytorch.py:1171-1294  -> se3_knn_fwd
+ *     (packed batches of clouds of different sizes, SE3Transformer.forward_packed: se3_knn_varlen_fwd; no reference counterpart)
  *   get_basis(r_ij, max_degree)                        basis.py:153-205                      -> se3_basis_fwd
  *   RadialFunc trunk (net.0 .. net.5)                  se3_transformer_pytorch.py:287-293    -> se3_radial_trunk_fwd
  *   PairwiseConv + ConvSE3 inner product               se3_transformer_pytorch.py:237-254,
@@ -54,6 +55,20 @@ int         se3_abi_version(void);
 int se3_knn_fwd(const float* coors, const uint8_t* node_mask, const uint8_t* neighbor_mask, const uint8_t* sparse_adj,
                 int b, int n, int k, float valid_radius, int causal,
                 int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream);
+
+/* Neighbour graph of a packed batch: clouds c = 0 .. num_clouds-1 of n_c = cu_seqlens[c+1] - cu_seqlens[c] nodes laid end to end,
+ * coors [total, 3].  Each cloud is searched on its own, exactly as se3_knn_fwd(b = 1, n = n_c, k = k_per_cloud[c]) with no node
+ * mask (same keys, tie rule, arithmetic and mask rule: the first k_c slots of a row are bit-identical to it), and the indices are
+ * global (start_c added).  Outputs have K >= max k_c slots per node: out_idx / out_mask / out_rel_dist [total, K],
+ * out_rel_pos [total, K, 3]; slots r >= k_c repeat slot k_c - 1 with mask 0.  neighbor_mask / sparse_adj: the clouds' [n_c, n_c]
+ * matrices flattened end to end ([sum n_c^2] uint8), pair (i, j) of cloud c at pair_off[c] + i n_c + j; either may be NULL
+ * (pair_off may be NULL when both are).  cu_seqlens [num_clouds+1] int64, k_per_cloud [num_clouds] int32, pair_off [num_clouds]
+ * int64 are DEVICE arrays; the call reads them back (one synchronisation of `stream`) and refuses n_c outside [2, 4097] or
+ * above max_len, k_c outside [1, n_c - 1], K < k_c and inconsistent offsets. */
+int se3_knn_varlen_fwd(const float* coors, const int64_t* cu_seqlens, const int* k_per_cloud, const uint8_t* neighbor_mask,
+                       const uint8_t* sparse_adj, const int64_t* pair_off, int num_clouds, int64_t total, int K, int max_len,
+                       float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos,
+                       float* out_rel_dist, void* stream);
 
 /* Gather per-pair features onto the neighbour list (batched_index_select at S:1293-1294, utils.py:56-70):
  * out[b,i,kk,:] = pair_feat[b,i,idx[b,i,kk],:]   with pair_feat [b,n,n,e]. */

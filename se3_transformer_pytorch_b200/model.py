@@ -8,6 +8,7 @@ libse3b200.so through `ops`; the cheap glue around it (embeddings, LinearSE3 GEM
 
 Forward only: everything runs under torch.no_grad().  CUDA only: there is no CPU fallback.
 """
+import operator
 import os
 from math import sqrt
 
@@ -1117,14 +1118,37 @@ class SE3Transformer(nn.Module):
                 neighbor_mask=None, global_feats=None):
         kw = dict(mask=mask, adj_mat=adj_mat, edges=edges, return_type=return_type, return_pooled=return_pooled,
                   neighbor_mask=neighbor_mask, global_feats=global_feats)
-        out, checks = self._forward_once(feats, coors, **kw)
+        return self._checked(lambda: self._forward_once(feats, coors, **kw))
+
+    @torch.no_grad()
+    def forward_packed(self, feats, coors, seqlens, adj_mat=None, edges=None, neighbor_mask=None, return_type=None,
+                       return_pooled=False):
+        """Clouds of different sizes in one forward, concatenated along the node axis instead of padded (no reference
+        counterpart; DESIGN.md section 7).  For every cloud c this returns what forward() returns for that cloud alone (batch 1,
+        no mask, its own pair inputs), concatenated along the node axis: each cloud keeps its own neighbour count
+        k_c = min(min(num_neighbors, n_c - 1) + min(max_sparse_neighbors, bonded_c), n_c - 1), and positions, rotary positions
+        and causal order count from the cloud's first node.  No edge of one cloud reaches another, and none is spent on padding.
+
+        feats: [T, dim_in] float, [T] long tokens (num_tokens) or {'d': [T, C_d, 2d+1]}; coors [T, 3];
+        seqlens: B node counts summing to T (1-D int tensor or sequence of ints), each in [2, 4097].
+        adj_mat, neighbor_mask: lists of B bool [n_c, n_c]; edges: list of B [n_c, n_c] long tokens or [n_c, n_c, edge_dim] float.
+        Returns {'d': [T, C, 2d+1]} ('0': [T, C]; reduce_dim_out drops C), or one of them with return_type; return_pooled gives
+        the per-cloud mean over nodes, [B, ...].  Models built with global_feats_dim are not supported."""
+        seqlens = self._check_packed(feats, coors, seqlens, adj_mat, edges, neighbor_mask)
+        return self._checked(lambda: self._forward_packed_once(feats, coors, seqlens, adj_mat, edges, neighbor_mask, return_type,
+                                                               return_pooled))
+
+    def _checked(self, once):
+        """Run one forward (once() -> (out, deferred low-rank checks)) and the run-time check of its low-rank plans; on a plan
+        miss the affected ConvSE3 move to the direct kernels and the forward runs again."""
+        out, checks = once()
         if torch.cuda.is_current_stream_capturing():
             self._graph_checks = checks               # static tensors of the graph: GraphedForward reads them after each replay
             return out
         bad = check_lowrank_stats(checks)             # the one host synchronisation of the low-rank plans, once per forward
         if bad:
             self.handle_plan_miss(bad)
-            out, checks = self._forward_once(feats, coors, **kw)
+            out, checks = once()
             assert not check_lowrank_stats(checks)
         return out
 
@@ -1144,20 +1168,10 @@ class SE3Transformer(nn.Module):
                       neighbor_mask=None, global_feats=None):
         assert not (self.accept_global_feats ^ exists(global_feats)), 'you cannot pass in global features unless you init the class correctly'
         _mask = mask
-        # float64 models / inputs (reference tests/test_equivariance.py:228-258 runs under a float64 default dtype): the kernels
-        # compute in float32; parameters are converted once, inputs are cast, results are returned in the caller's dtype
-        out_dtype = coors.dtype if coors.dtype == torch.float64 else None
-        if any(p.dtype == torch.float64 for p in self.parameters()):
-            import warnings
-            warnings.warn('se3_transformer_pytorch_b200 computes in float32: converting the float64 parameters of this model to float32')
-            self.float()
+        out_dtype = self._compute_dtype(coors)
         if self.output_degrees == 1:
             return_type = 0
-        if exists(self.token_emb):
-            feats = self.token_emb(feats)
-        if exists(self.pos_emb):
-            assert feats.shape[1] <= self.num_positions, 'feature sequence length must be less than the number of positions given at init'
-            feats = feats + self.pos_emb(torch.arange(feats.shape[1], device=feats.device)).unsqueeze(0)
+        feats = self._embed_tokens(feats)
         assert not (self.attend_sparse_neighbors and not exists(adj_mat)), 'adjacency matrix (adjacency_mat) or edges (edges) must be passed in'
         assert not (self.has_edges and not exists(edges)), 'edge embedding (num_edge_tokens & edge_dim) must be supplied if one were to train on edge types'
         if torch.is_tensor(feats):
@@ -1168,17 +1182,82 @@ class SE3Transformer(nn.Module):
             global_feats = {k: v.float() for k, v in global_feats.items()}
         if exists(edges) and edges.is_floating_point():
             edges = edges.float()
-        b, n, d = feats['0'].shape[:3]
+        b, n = feats['0'].shape[:2]
         device = feats['0'].device
-        if not coors.is_cuda:
-            raise RuntimeError('se3_transformer_pytorch_b200 runs on CUDA (sm_90a) only; move the model and inputs to the GPU')
-        assert d == self.dim_in[0], f'feature dimension {d} must be equal to dimension given at init {self.dim_in[0]}'
-        assert set(map(int, feats.keys())) == set(range(self.input_degrees)), f'input must have {self.input_degrees} degree'
-        feats = {k: v.float().contiguous() for k, v in feats.items()}
-        neighbors, max_sparse, valid_radius = self.num_neighbors, self.max_sparse_neighbors, self.valid_radius
+        feats = self._check_features(feats, coors)
+        neighbors, valid_radius = self.num_neighbors, self.valid_radius
         assert self.attend_sparse_neighbors or neighbors > 0, 'you must either attend to sparsely bonded neighbors, or set number of locally attended neighbors to be greater than 0'
 
+        adj_indices, sparse_mask, num_sparse = self._bonded(adj_mat, b, n, device)
+        if neighbors == 0:
+            valid_radius = 0
+        k_local = int(min(neighbors, n - 1))
+        total = int(k_local + num_sparse)
+        assert total > 0, 'you must be fetching at least 1 neighbor'
+        total = int(min(total, n - 1))
+        if exists(neighbor_mask):
+            self._report_neighbor_mask(neighbor_mask, n)
+
+        idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=neighbor_mask,
+                                                sparse_adj=sparse_mask, causal=self.causal)
+
+        # edge features on the neighbour list (reference S:1231-1239, 1293-1294); gather first, embed after
+        e = None
+        if exists(edges):
+            if exists(self.edge_emb):
+                if edges.dim() == 2:                            # [b, n] tokens: the reference broadcasts them over rows (b == 1)
+                    assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
+                    edges = edges.unsqueeze(1).expand(b, n, n)
+                e = self.edge_emb(edges.gather(2, idx))
+            else:
+                e = ops.gather_pairs(edges.float(), idx)
+        if exists(self.adj_emb):
+            a = self.adj_emb(adj_indices.gather(2, idx))
+            e = torch.cat((e, a), dim=-1) if exists(e) else a
+
+        pos_emb = None
+        if exists(self.rotary_pos_emb):
+            pos = torch.arange(n, device=device)
+            pos_emb = self._rotary(pos.view(1, n).expand(b, n), torch.cat((pos.view(1, n, 1).expand(b, n, 1), idx), dim=2), n, rel_dist)
+        pool = None
+        if return_pooled:
+            pool = lambda v: masked_mean_nodes(v, _mask) if exists(_mask) else v.mean(dim=1)
+        return self._trunk(feats, (idx, nmask, e), rel_pos, rel_dist, pos_emb, global_feats, _mask, pool, out_dtype, return_type)
+
+    # ---- pieces shared by forward and forward_packed -------------------------------------------------------
+    def _compute_dtype(self, coors):
+        """float64 models / inputs (reference tests/test_equivariance.py:228-258 runs under a float64 default dtype): the kernels
+        compute in float32; parameters are converted once, inputs are cast, results are returned in the caller's dtype."""
+        if any(p.dtype == torch.float64 for p in self.parameters()):
+            import warnings
+            warnings.warn('se3_transformer_pytorch_b200 computes in float32: converting the float64 parameters of this model to float32')
+            self.float()
+        return coors.dtype if coors.dtype == torch.float64 else None
+
+    def _embed_tokens(self, feats, positions=None):
+        """Token and absolute-position embeddings (reference S:1149-1160) of feats [b, n, ...]; positions [n] (default 0 .. n-1)."""
+        if exists(self.token_emb):
+            feats = self.token_emb(feats)
+        if exists(self.pos_emb):
+            if positions is None:
+                assert feats.shape[1] <= self.num_positions, 'feature sequence length must be less than the number of positions given at init'
+                positions = torch.arange(feats.shape[1], device=feats.device)
+            feats = feats + self.pos_emb(positions).unsqueeze(0)
+        return feats
+
+    def _check_features(self, feats, coors):
+        if not coors.is_cuda:
+            raise RuntimeError('se3_transformer_pytorch_b200 runs on CUDA (sm_90a) only; move the model and inputs to the GPU')
+        d = feats['0'].shape[2]
+        assert d == self.dim_in[0], f'feature dimension {d} must be equal to dimension given at init {self.dim_in[0]}'
+        assert set(map(int, feats.keys())) == set(range(self.input_degrees)), f'input must have {self.input_degrees} degree'
+        return {k: v.float().contiguous() for k, v in feats.items()}
+
+    def _bonded(self, adj_mat, b, n, device):
+        """N-hop adjacency (reference S:1177-1191) and the bonded neighbours (S:1198-1217) of clouds of n nodes: returns
+        (adj_indices [b, n, n] hop counts or None, sparse_mask [b, n, n] or None, num_sparse)."""
         eye = torch.eye(n, dtype=torch.bool, device=device)
+        max_sparse = self.max_sparse_neighbors
         adj_indices = None
         if exists(self.num_adj_degrees):                       # N-hop adjacency, reference S:1177-1191
             if adj_mat.dim() == 2:
@@ -1209,63 +1288,47 @@ class SE3Transformer(nn.Module):
             else:
                 sparse_mask = torch.zeros_like(adj_vals, dtype=torch.bool)
 
-        if neighbors == 0:
-            valid_radius = 0
-        k_local = int(min(neighbors, n - 1))
-        total = int(k_local + num_sparse)
-        assert total > 0, 'you must be fetching at least 1 neighbor'
-        total = int(min(total, n - 1))
-        if exists(neighbor_mask):
-            max_nb = int(neighbor_mask.masked_fill(eye.unsqueeze(0), False).sum(dim=-1).max().item())
-            if max_nb > neighbors:
-                print(f'neighbor_mask shows maximum number of neighbors as {max_nb} but specified number of neighbors is {neighbors}')
+        return adj_indices, sparse_mask, num_sparse
 
-        idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=neighbor_mask,
-                                                sparse_adj=sparse_mask, causal=self.causal)
+    def _report_neighbor_mask(self, neighbor_mask, n):
+        eye = torch.eye(n, dtype=torch.bool, device=neighbor_mask.device)
+        max_nb = int(neighbor_mask.masked_fill(eye.unsqueeze(0), False).sum(dim=-1).max().item())
+        if max_nb > self.num_neighbors:
+            print(f'neighbor_mask shows maximum number of neighbors as {max_nb} but specified number of neighbors is {self.num_neighbors}')
 
-        # edge features on the neighbour list (reference S:1231-1239, 1293-1294); gather first, embed after
-        e = None
-        if exists(edges):
-            if exists(self.edge_emb):
-                if edges.dim() == 2:                            # [b, n] tokens: the reference broadcasts them over rows (b == 1)
-                    assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
-                    edges = edges.unsqueeze(1).expand(b, n, n)
-                e = self.edge_emb(edges.gather(2, idx))
-            else:
-                e = ops.gather_pairs(edges.float(), idx)
-        if exists(self.adj_emb):
-            a = self.adj_emb(adj_indices.gather(2, idx))
-            e = torch.cat((e, a), dim=-1) if exists(e) else a
+    def _rotary(self, q_pos, k_pos, n_pos, rel_dist):
+        """Rotary embeddings of the type-0 queries and keys (reference S:1298-1325): q_pos [b, n] and k_pos [b, n, 1 + k] (self
+        first) are node positions inside their cloud, all below n_pos; rel_dist [b, n, k]."""
+        q_parts, k_parts = [], []
+        if self.rotary_position:
+            seq_emb = self.rotary_pos_emb(torch.arange(n_pos, device=q_pos.device))                # [n_pos, d]
+            k_parts.append(seq_emb[k_pos])                                                          # [b, n, 1 + k, d]
+            q_parts.append(seq_emb[q_pos])
+        if self.rotary_rel_dist:
+            k_parts.append(self.rotary_pos_emb(F.pad(rel_dist, (1, 0), value=0.) * 1e2))
+            q_parts.append(self.rotary_pos_emb(torch.zeros(q_pos.shape, device=q_pos.device)))
+        return torch.cat(q_parts, dim=-1), torch.cat(k_parts, dim=-1)
 
+    def _trunk(self, feats, edge_info, rel_pos, rel_dist, pos_emb, global_feats, mask, reduce, out_dtype, return_type):
+        """Everything after the graph (reference S:1240-1375): conv_in, pre-convs, attention blocks, conv_out, norm, linear_out
+        and the output format.  reduce (or None) maps every output [b, n, ...] to what is returned (pooling, unbatching).
+        Returns (output, the deferred run-time checks of the low-rank plans)."""
         geom = Geometry(rel_pos, self.num_degrees - 1)
         geom.deferred = []
         basis = ops.basis_flat(rel_pos, self.num_degrees - 1) + (geom,)
-        edge_info = (idx, nmask, e)
         x = self.conv_in(feats, edge_info, rel_dist=rel_dist, basis=basis)
         for conv, nonlin in self.convs:
             x = nonlin(x)
             x = conv(x, edge_info, rel_dist=rel_dist, basis=basis)
-        pos_emb = None
-        if exists(self.rotary_pos_emb):                         # reference S:1298-1325
-            q_parts, k_parts = [], []
-            if self.rotary_position:
-                seq_emb = self.rotary_pos_emb(torch.arange(n, device=device))                       # [n, d]
-                with_self = torch.cat((torch.arange(n, device=device).view(1, n, 1).expand(b, n, 1), idx), dim=2)
-                k_parts.append(seq_emb[with_self])                                                   # [b, n, 1 + k, d]
-                q_parts.append(seq_emb.unsqueeze(0).expand(b, n, -1))
-            if self.rotary_rel_dist:
-                k_parts.append(self.rotary_pos_emb(F.pad(rel_dist, (1, 0), value=0.) * 1e2))
-                q_parts.append(self.rotary_pos_emb(torch.zeros(n, device=device)).unsqueeze(0).expand(b, n, -1))
-            pos_emb = (torch.cat(q_parts, dim=-1), torch.cat(k_parts, dim=-1))
-        x = self.net(x, edge_info=edge_info, rel_dist=rel_dist, basis=basis, global_feats=global_feats, pos_emb=pos_emb, mask=_mask)
+        x = self.net(x, edge_info=edge_info, rel_dist=rel_dist, basis=basis, global_feats=global_feats, pos_emb=pos_emb, mask=mask)
         if exists(self.conv_out):
             x = self.conv_out(x, edge_info, rel_dist=rel_dist, basis=basis)
         x = self.norm(x)
         if exists(self.linear_out):
             x = self.linear_out(x)
             x = {k: v.squeeze(dim=2) for k, v in x.items()}
-        if return_pooled:
-            x = {k: (masked_mean_nodes(v, _mask) if exists(_mask) else v.mean(dim=1)) for k, v in x.items()}
+        if exists(reduce):
+            x = {k: reduce(v) for k, v in x.items()}
         if '0' in x:
             x['0'] = x['0'].squeeze(dim=-1)
         if exists(out_dtype):
@@ -1273,6 +1336,114 @@ class SE3Transformer(nn.Module):
         if exists(return_type):
             return x[str(return_type)], geom.deferred
         return x, geom.deferred
+
+    # ---- packed batches ------------------------------------------------------------------------------------
+    def _check_packed(self, feats, coors, seqlens, adj_mat, edges, neighbor_mask):
+        """Everything forward_packed takes from the caller, checked before any device work; returns seqlens as a list of ints."""
+        if self.accept_global_feats:
+            raise NotImplementedError('forward_packed: models built with global_feats_dim are not supported (the attention kernel '
+                                      'indexes the global keys by batch row, and a packed batch is one row)')
+        if torch.is_tensor(seqlens):
+            if seqlens.dim() != 1 or seqlens.is_floating_point() or seqlens.is_complex() or seqlens.dtype == torch.bool:
+                raise ValueError(f'forward_packed: seqlens must be a 1-D integer tensor, got {seqlens.dtype} of shape {tuple(seqlens.shape)}')
+            seqlens = seqlens.tolist()
+        try:
+            seqlens = [operator.index(n) for n in seqlens]
+        except TypeError:
+            raise ValueError('forward_packed: seqlens must be a 1-D integer tensor or a sequence of ints') from None
+        if not seqlens:
+            raise ValueError('forward_packed: seqlens is empty')
+        B, T = len(seqlens), sum(seqlens)
+        for t in (feats.values() if isinstance(feats, dict) else [feats]):
+            if not torch.is_tensor(t) or t.dim() < 1 or t.shape[0] != T:
+                raise ValueError(f'forward_packed: the features must have sum(seqlens) = {T} rows, got '
+                                 f'{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}')
+        if not torch.is_tensor(coors) or tuple(coors.shape) != (T, 3):
+            raise ValueError(f'forward_packed: coors must be [sum(seqlens), 3] = {(T, 3)}, got '
+                             f'{tuple(coors.shape) if torch.is_tensor(coors) else type(coors).__name__}')
+        bad = [n for n in seqlens if not 2 <= n <= ops.MAX_CLOUD]
+        if bad:
+            raise ValueError(f'forward_packed: every cloud needs 2 .. {ops.MAX_CLOUD} nodes, got {bad[:8]}')
+        for name, per_cloud in (('adj_mat', adj_mat), ('edges', edges), ('neighbor_mask', neighbor_mask)):
+            if per_cloud is None:
+                continue
+            if not isinstance(per_cloud, (list, tuple)) or len(per_cloud) != B:
+                raise ValueError(f'forward_packed: {name} must be a list of {B} per-cloud tensors, got '
+                                 f'{len(per_cloud) if isinstance(per_cloud, (list, tuple)) else type(per_cloud).__name__}')
+            dims = 3 if name == 'edges' and not exists(self.edge_emb) else 2
+            for c, (t, n) in enumerate(zip(per_cloud, seqlens)):
+                if not torch.is_tensor(t) or t.dim() != dims or tuple(t.shape[:2]) != (n, n):
+                    want = f'[{n}, {n}, edge_dim]' if dims == 3 else f'[{n}, {n}]'
+                    raise ValueError(f'forward_packed: {name}[{c}] must be {want} for a cloud of {n} nodes, got '
+                                     f'{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}')
+        assert not (self.attend_sparse_neighbors and not exists(adj_mat)), 'adjacency matrix (adjacency_mat) or edges (edges) must be passed in'
+        assert not (self.has_edges and not exists(edges)), 'edge embedding (num_edge_tokens & edge_dim) must be supplied if one were to train on edge types'
+        if exists(self.pos_emb):
+            assert max(seqlens) <= self.num_positions, 'feature sequence length must be less than the number of positions given at init'
+        return seqlens
+
+    def _forward_packed_once(self, feats, coors, seqlens, adj_mat, edges, neighbor_mask, return_type, return_pooled):
+        out_dtype = self._compute_dtype(coors)
+        if self.output_degrees == 1:
+            return_type = 0
+        T, dev = sum(seqlens), coors.device
+        lens = torch.tensor(seqlens)
+        node_len = torch.repeat_interleave(lens, lens)                                  # n_c of every node
+        node_start = torch.repeat_interleave(lens.cumsum(0) - lens, lens)               # start_c of every node
+        local_pos = torch.arange(T) - node_start                                        # i_local
+        pair_row = torch.repeat_interleave(torch.tensor(ops.pair_offsets(seqlens)), lens) + local_pos * node_len - node_start
+        node_start, local_pos = node_start.to(dev), local_pos.to(dev)
+
+        if isinstance(feats, dict):
+            feats = {k: v.unsqueeze(0) for k, v in feats.items()}
+        else:
+            feats = self._embed_tokens(feats.unsqueeze(0), local_pos)
+            feats = {'0': feats[..., None]}
+        feats = self._check_features(feats, coors)
+        neighbors, valid_radius = self.num_neighbors, self.valid_radius
+        assert self.attend_sparse_neighbors or neighbors > 0, 'you must either attend to sparsely bonded neighbors, or set number of locally attended neighbors to be greater than 0'
+        if neighbors == 0:
+            valid_radius = 0
+
+        # per cloud, exactly as forward() on that cloud alone: bonded neighbours, hop counts and the neighbour count k_c
+        ks, sparse, hops = [], [], []
+        for c, n in enumerate(seqlens):
+            adj_indices, sparse_mask, num_sparse = self._bonded(adj_mat[c].to(dev) if exists(adj_mat) else None, 1, n, dev)
+            total = int(int(min(neighbors, n - 1)) + num_sparse)
+            assert total > 0, 'you must be fetching at least 1 neighbor'
+            ks.append(int(min(total, n - 1)))
+            if exists(sparse_mask):
+                sparse.append(sparse_mask.reshape(-1))
+            if exists(adj_indices):
+                hops.append(adj_indices.reshape(-1))
+            if exists(neighbor_mask):
+                self._report_neighbor_mask(neighbor_mask[c].to(dev).unsqueeze(0), n)
+        nbr = torch.cat([m.to(dev).reshape(-1) for m in neighbor_mask]) if exists(neighbor_mask) else None
+        idx, nmask, rel_pos, rel_dist = ops.knn_varlen(coors.float(), seqlens, ks, max(ks), valid_radius, neighbor_mask=nbr,
+                                                       sparse_adj=torch.cat(sparse) if sparse else None, causal=self.causal)
+
+        # edge features: pair (i, j) of cloud c sits at pair_off[c] + i_local n_c + j_local of the flattened per-cloud inputs
+        e = None
+        if exists(edges) or exists(self.adj_emb):
+            flat = pair_row.to(dev)[:, None] + idx                                      # [T, K]
+        if exists(edges):
+            pf = torch.cat([t.to(dev).reshape(n * n, *t.shape[2:]) for t, n in zip(edges, seqlens)])
+            e = self.edge_emb(pf[flat]) if exists(self.edge_emb) else pf.float()[flat]
+        if exists(self.adj_emb):
+            a = self.adj_emb(torch.cat(hops)[flat])
+            e = torch.cat((e, a), dim=-1) if exists(e) else a
+
+        idx, nmask, rel_pos, rel_dist = idx.unsqueeze(0), nmask.unsqueeze(0), rel_pos.unsqueeze(0), rel_dist.unsqueeze(0)
+        pos_emb = None
+        if exists(self.rotary_pos_emb):
+            k_pos = torch.cat((local_pos.view(1, T, 1), idx - node_start.view(1, T, 1)), dim=2)
+            pos_emb = self._rotary(local_pos.view(1, T), k_pos, max(seqlens), rel_dist)
+        if return_pooled:
+            reduce = lambda v: torch.stack([s.mean(dim=0) for s in v[0].split(seqlens)])
+        else:
+            reduce = lambda v: v[0]
+        edge_info = (idx, nmask, None if e is None else e.unsqueeze(0))
+        return self._trunk(feats, edge_info, rel_pos, rel_dist, pos_emb, None, None, reduce, out_dtype, return_type)
 
 
 class GraphedForward:

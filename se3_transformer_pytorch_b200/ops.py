@@ -23,6 +23,7 @@ _SIGNATURES = {
     'se3_last_error': (ctypes.c_char_p, []),
     'se3_abi_version': (c_int, []),
     'se3_knn_fwd': (c_int, [c_void_p] * 4 + [c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
+    'se3_knn_varlen_fwd': (c_int, [c_void_p] * 6 + [c_int, c_int64, c_int, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
     'se3_radial_trunk_fwd': (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -167,6 +168,55 @@ def knn(coors, k, valid_radius, node_mask=None, neighbor_mask=None, sparse_adj=N
     with torch.cuda.device(coors.device), _timed('knn', nbytes=nbytes):
         _check(lib().se3_knn_fwd(_p(coors), _p(nm), _p(nbm), _p(sa), b, n, k, valid_radius, int(bool(causal)),
                                  _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
+    return idx, mask.view(torch.bool), rel_pos, rel_dist
+
+
+MAX_CLOUD = 4097      # nodes per cloud of the shared-memory sort (n - 1 <= 4096 columns)
+
+
+def pair_offsets(seqlens):
+    """Start of each cloud's [n_c, n_c] block in a flattened packed pair input: sum of n_c'^2 over the clouds before it."""
+    off = [0]
+    for n in seqlens[:-1]:
+        off.append(off[-1] + n * n)
+    return off
+
+
+def knn_varlen(coors, seqlens, k_per_cloud, K, valid_radius, neighbor_mask=None, sparse_adj=None, causal=False):
+    """Neighbour graph of a packed batch (SE3Transformer.forward_packed): clouds of seqlens[c] nodes laid end to end in
+    coors [T, 3], each searched on its own for k_per_cloud[c] neighbours, K >= max k_c slots per node (slots past k_c repeat
+    slot k_c - 1, masked).  neighbor_mask / sparse_adj: the clouds' [n_c, n_c] matrices flattened end to end ([sum n_c^2]).
+    Returns idx int64 [T, K] (global node indices), mask bool [T, K], rel_pos [T, K, 3], rel_dist [T, K]."""
+    _require_cuda(coors, neighbor_mask, sparse_adj)
+    coors = _f32(coors)
+    seqlens, k_per_cloud = [int(v) for v in seqlens], [int(v) for v in k_per_cloud]
+    B, T = len(seqlens), sum(seqlens)
+    if B == 0 or coors.shape != (T, 3):
+        raise ValueError(f'knn_varlen: coors must be [sum(seqlens), 3] = {(T, 3)} for {B} clouds, got {tuple(coors.shape)}')
+    if len(k_per_cloud) != B:
+        raise ValueError(f'knn_varlen: k_per_cloud has {len(k_per_cloud)} entries for {B} clouds')
+    if min(seqlens) < 2 or max(seqlens) > MAX_CLOUD:
+        raise ValueError(f'knn_varlen: every cloud needs 2 .. {MAX_CLOUD} nodes, got lengths {min(seqlens)} .. {max(seqlens)}')
+    if any(not 1 <= kc <= n - 1 for kc, n in zip(k_per_cloud, seqlens)) or K < max(k_per_cloud):
+        raise ValueError(f'knn_varlen: need 1 <= k_c <= n_c - 1 and K >= max k_c (K = {K}, k = {k_per_cloud}, n = {seqlens})')
+    npairs = sum(n * n for n in seqlens)
+    for name, t in (('neighbor_mask', neighbor_mask), ('sparse_adj', sparse_adj)):
+        if t is not None and t.shape != (npairs,):
+            raise ValueError(f'knn_varlen: {name} must be the flattened per-cloud [n_c, n_c] matrices, [{npairs}], got {tuple(t.shape)}')
+    dev = coors.device
+    cu = torch.tensor([0] + seqlens, dtype=torch.int64).cumsum(0).to(dev)
+    kc = torch.tensor(k_per_cloud, dtype=torch.int32).to(dev)
+    nbm, sa = _u8(neighbor_mask), _u8(sparse_adj)
+    off = torch.tensor(pair_offsets(seqlens), dtype=torch.int64).to(dev) if nbm is not None or sa is not None else None
+    idx = torch.empty((T, K), dtype=torch.int64, device=dev)
+    mask = torch.empty((T, K), dtype=torch.uint8, device=dev)
+    rel_pos = torch.empty((T, K, 3), dtype=torch.float32, device=dev)
+    rel_dist = torch.empty((T, K), dtype=torch.float32, device=dev)
+    valid_radius = float(min(valid_radius, 3.0e38))
+    nbytes = 12 * T + 25 * T * K + sum(t.numel() for t in (nbm, sa) if t is not None)
+    with torch.cuda.device(dev), _timed('knn_varlen', nbytes=nbytes):
+        _check(lib().se3_knn_varlen_fwd(_p(coors), _p(cu), _p(kc), _p(nbm), _p(sa), _p(off), B, T, K, max(seqlens), valid_radius,
+                                        int(bool(causal)), _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
     return idx, mask.view(torch.bool), rel_pos, rel_dist
 
 
