@@ -287,9 +287,11 @@ class ConvSE3(nn.Module):
         return torch.cat([xs.sin(), xs.cos(), rd], dim=-1)
 
     def lowrank_plan(self, d_max):
-        """Per pair: orthonormal V [128, r] spanning the curve g(d), d in [0, D], and the tensor-core image of
-        F'' = [W3 V | b3 | 0].  Depends on the weights and on D only: built once (and again if weights change or a forward
-        brings a larger distance).  Only for distance-only radial functions (no extra edge features)."""
+        """Per pair: orthonormal V [128, r] spanning the curve g(d), d in [0, D], and the tensor-core images of F'' = [W3 V | b3 | 0]
+        in the pair's formulation `kind`: if every pair has a plan, 'z' (in the per-(degree_out, |m|) GEMM images plan['z'],
+        DESIGN.md 4.5) or 'aligned' (one image per |m|, 4.4); otherwise 'input_side' (one image per frequency, 4.3) or 'combined'
+        (4.2).  Depends on the weights and on D only: built once (and again if weights change or a forward brings a larger
+        distance).  Only for distance-only radial functions (no extra edge features)."""
         pk = self.packed()
         plan = pk.get('lr')
         if plan is not None and plan['D'] >= d_max:
@@ -298,83 +300,89 @@ class ConvSE3(nn.Module):
         D = 1.25 * d_max
         with torch.no_grad():
             grid = torch.linspace(0.0, D, self.LR_GRID, device=dev, dtype=torch.float64).unsqueeze(-1)
-            feat = self.encode_dist(grid)
-            pairs = {}
-            bases = {}
-            ugrid = {}
-            for di, do in self.pairs:
-                pc = self.kernel_unary[f'({di},{do})']
-                if self.tc_eligible(di, do) and pc.rp.net['6'].weight.numel() > 0:
-                    G64 = pc.rp.trunk64(feat)
-                    basis = ops.lowrank_basis(G64)
-                    if basis is not None:
-                        bases[(di, do)] = basis
-                        ugrid[(di, do)] = ((G64 - basis[2]) @ basis[1], float(G64.abs().max()))     # U(d) on the grid, float64
-                    del G64
-            # the edge-aligned images serve a ConvSE3 only if EVERY pair has a plan (all launches of an output degree then
-            # accumulate in the aligned frame); otherwise keep the global-frame images of 4.2-4.3 for the covered pairs
-            aligned_images = use_aligned() and len(bases) == len(self.pairs)
-            zplan = None
-            if aligned_images and use_zgemm() and self.zgemm_eligible({pair: 16 * ((rv[0] + 1 + 15) // 16) for pair, rv in bases.items()}):
-                zplan = {}                    # (do, m) -> dict(img, degs): one GEMM per output degree and |m| (DESIGN.md 4.5)
-                fps = {}
-            for (di, do), (r, V, gmean) in bases.items():
-                pc = self.kernel_unary[f'({di},{do})']
-                lin = pc.rp.net['6']
-                Kp = 16 * ((r + 1 + 15) // 16)
-                Fp = torch.zeros((lin.weight.shape[0], Kp), dtype=torch.float32, device=dev)
+            bases, ugrid = self._factor_curves(self.encode_dist(grid))
+            complete = len(bases) == len(self.pairs)
+            aligned = use_aligned() and complete
+            z = aligned and use_zgemm() and self.zgemm_eligible({pair: lowrank_k(rv[0]) for pair, rv in bases.items()})
+            pairs, zweights = {}, {}
+            for pair, (r, V, gmean) in bases.items():
+                kind = 'z' if z else 'aligned' if aligned else 'input_side' if input_side(*pair) else 'combined'
+                lin = self.kernel_unary[f'({pair[0]},{pair[1]})'].rp.net['6']
+                Fp = torch.zeros((lin.weight.shape[0], lowrank_k(r)), dtype=torch.float32, device=dev)
                 Fp[:, :r] = (lin.weight.double() @ V).float()
                 Fp[:, r] = (lin.bias.double() + lin.weight.double() @ gmean).float()      # affine model: W3 gmean joins the bias
+                if kind == 'z':
+                    zweights[pair] = self.aligned_weights(pair, Fp)
                 Vp = torch.zeros((ops.RADIAL_MID, 64), dtype=torch.float32, device=dev)
                 Vp[:, :r] = V.float()
-                if zplan is not None:
-                    # the aligned weights w0, (a_m, b_m) = constant combinations of the F frequencies (rows (o,i,f) of F'); they are
-                    # concatenated over the input degrees into one GEMM image per (do, m) below
-                    Fv = Fp.view(pc.nc_out, pc.nc_in, pc.num_freq, Kp).double()
-                    c0, ca, cb = (t.to(dev) for t in _aligned.aligned_coeffs(di, do))
-                    fps[(di, do, 0)] = torch.einsum('oifk,f->oik', Fv, c0).reshape(-1, Kp).float().contiguous()
-                    for m in range(1, min(di, do) + 1):
-                        ab = torch.stack([torch.einsum('oifk,f->oik', Fv, ca[m - 1]), torch.einsum('oifk,f->oik', Fv, cb[m - 1])], dim=2)
-                        fps[(di, do, m)] = ab.reshape(-1, Kp).float().contiguous()
-                    pairs[(di, do)] = dict(r=r, Kp=Kp, V=Vp, gmean=gmean.float(), img=None, imgs_f=None, al_imgs=None, z=True)
-                    del Fv
-                elif aligned_images:
-                    # edge-aligned formulation (DESIGN.md 4.4): images of the weights a_m, b_m = constant combinations of the
-                    # F frequencies (rows (o,i,f) of F'), one image per m
-                    Fv = Fp.view(pc.nc_out, pc.nc_in, pc.num_freq, Kp).double()
-                    c0, ca, cb = (t.to(dev) for t in _aligned.aligned_coeffs(di, do))
-                    imgs = [ops.pack_lowrank(torch.einsum('oifk,f->oik', Fv, c0).reshape(-1, Kp).float().contiguous(),
-                                             pc.nc_out, pc.nc_in, 1, Kp)]
-                    for m in range(1, min(di, do) + 1):
-                        ab = torch.stack([torch.einsum('oifk,f->oik', Fv, ca[m - 1]), torch.einsum('oifk,f->oik', Fv, cb[m - 1])], dim=2)
-                        imgs.append(ops.pack_lowrank(ab.reshape(-1, Kp).float().contiguous(), pc.nc_out, pc.nc_in, 2, Kp))
-                    pairs[(di, do)] = dict(r=r, Kp=Kp, V=Vp, gmean=gmean.float(), img=None, imgs_f=None, al_imgs=imgs)
-                    del Fv
-                elif input_side(di, do) and pc.num_freq > 1:
-                    # input-side contraction (DESIGN.md 4.3): one image per frequency f (rows (o,i,f) of F'), no combined image
-                    Fv = Fp.view(pc.nc_out, pc.nc_in, pc.num_freq, Kp)
-                    imgs = [ops.pack_lowrank(Fv[:, :, f, :].reshape(-1, Kp).contiguous(), pc.nc_out, pc.nc_in, 1, Kp)
-                            for f in range(pc.num_freq)]
-                    pairs[(di, do)] = dict(r=r, Kp=Kp, V=Vp, gmean=gmean.float(), img=None, imgs_f=imgs)
-                else:
-                    img = ops.pack_lowrank(Fp, pc.nc_out, pc.nc_in, pc.num_freq, Kp)
-                    pairs[(di, do)] = dict(r=r, Kp=Kp, V=Vp, gmean=gmean.float(), img=img, imgs_f=[img] if pc.num_freq == 1 else None)
-                del Fp
-            if zplan is not None:
-                for do, mo in self.fiber_out:
-                    for m in range(do + 1):
-                        degs = [(di, mi) for di, mi in self.fiber_in if di >= m]
-                        if not degs:
-                            continue
-                        mode = 1 if m == 0 else z_mode_m()
-                        img, S = ops.zgemm_image([(fps.pop((di, do, m)), mi) for di, mi in degs], mo, mode)
-                        zplan[(do, m)] = dict(img=img, S=S, degs=degs, mode=mode)
-                del fps
-            utab = self.radial_table(ugrid, bases, grid, dev) if len(bases) == len(self.pairs) and use_utable() else None
-            del ugrid
-        plan = dict(D=D, pairs=pairs, z=zplan, utab=utab)
+                pairs[pair] = dict(kind=kind, r=r, Kp=Fp.shape[1], V=Vp, gmean=gmean.float(),
+                                   images=[] if kind == 'z' else self._pack_images(pair, kind, Fp))
+            zplan = self._zgemm_images(zweights) if z else None
+            utab = self.radial_table(ugrid, bases, grid, dev) if complete and use_utable() else None
+            plan = dict(D=D, pairs=pairs, z=zplan, utab=utab, **self._plan_stacks(pairs, dev))
         pk['lr'] = plan
         return plan
+
+    def _factor_curves(self, feat):
+        """Every tc-eligible pair that still has its net.6 weights and whose curve g(d) (float64 trunk on the distance grid
+        `feat`) has a low-rank model: {pair: (r, V, gmean)} and {pair: (U(d) = (g - gmean) V on the grid, max|g|)}."""
+        bases, ugrid = {}, {}
+        for di, do in self.pairs:
+            pc = self.kernel_unary[f'({di},{do})']
+            if self.tc_eligible(di, do) and pc.rp.net['6'].weight.numel() > 0:
+                G64 = pc.rp.trunk64(feat)
+                basis = ops.lowrank_basis(G64)
+                if basis is not None:
+                    bases[(di, do)] = basis
+                    ugrid[(di, do)] = ((G64 - basis[2]) @ basis[1], float(G64.abs().max()))
+        return bases, ugrid
+
+    def aligned_weights(self, pair, Fp):
+        """The edge-aligned weights [w0, (a_m, b_m) for m = 1..min(di, do)] (DESIGN.md 4.4): constant combinations of the F
+        frequencies (rows (o,i,f) of F'), as [Co*Ci, Kp] (m = 0) and [Co*Ci*2, Kp] (rows (o,i,(a,b))) fp32 matrices."""
+        di, do = pair
+        pc = self.kernel_unary[f'({di},{do})']
+        Kp = Fp.shape[1]
+        Fv = Fp.view(pc.nc_out, pc.nc_in, pc.num_freq, Kp).double()
+        c0, ca, cb = (t.to(Fp.device) for t in _aligned.aligned_coeffs(di, do))
+        ws = [torch.einsum('oifk,f->oik', Fv, c0).reshape(-1, Kp).float().contiguous()]
+        for m in range(1, min(di, do) + 1):
+            ab = torch.stack([torch.einsum('oifk,f->oik', Fv, ca[m - 1]), torch.einsum('oifk,f->oik', Fv, cb[m - 1])], dim=2)
+            ws.append(ab.reshape(-1, Kp).float().contiguous())
+        return ws
+
+    def _pack_images(self, pair, kind, Fp):
+        """pairwise_lr images of one pair in formulation `kind` (see lowrank_plan)."""
+        pc = self.kernel_unary[f'({pair[0]},{pair[1]})']
+        Co, Ci, nf, Kp = pc.nc_out, pc.nc_in, pc.num_freq, Fp.shape[1]
+        if kind == 'aligned':
+            return [ops.pack_lowrank(w, Co, Ci, 1 if m == 0 else 2, Kp) for m, w in enumerate(self.aligned_weights(pair, Fp))]
+        if kind == 'input_side':
+            Fv = Fp.view(Co, Ci, nf, Kp)
+            return [ops.pack_lowrank(Fv[:, :, f, :].reshape(-1, Kp).contiguous(), Co, Ci, 1, Kp) for f in range(nf)]
+        return [ops.pack_lowrank(Fp, Co, Ci, nf, Kp)]
+
+    def _zgemm_images(self, zweights):
+        """{(do, m): dict(img, S, degs, mode)}: the aligned weights of the pairs (di >= m, do) as one GEMM image (DESIGN.md 4.5)."""
+        zplan = {}
+        for do, mo in self.fiber_out:
+            for m in range(do + 1):
+                degs = [(di, mi) for di, mi in self.fiber_in if di >= m]
+                if not degs:
+                    continue
+                mode = 1 if m == 0 else z_mode_m()
+                img, S = ops.zgemm_image([(zweights[(di, do)][m], mi) for di, mi in degs], mo, mode)
+                zplan[(do, m)] = dict(img=img, S=S, degs=degs, mode=mode)
+        return zplan
+
+    def _plan_stacks(self, pairs, dev):
+        """Operands of the radial kernels over all pairs (zero where a pair has no plan): Vstack [pairs, 128, 64], gmean
+        [pairs, 128], ones_col [pairs] (the column of U that holds 1) and have [pairs] (the pair is in the plan)."""
+        pps = [pairs.get(pair) for pair in self.pairs]
+        Vs = torch.stack([pp['V'] if pp else torch.zeros((ops.RADIAL_MID, 64), device=dev) for pp in pps])
+        gm = torch.stack([pp['gmean'] if pp else torch.zeros(ops.RADIAL_MID, device=dev) for pp in pps])
+        return dict(Vstack=Vs, gmean=gm, ones_col=torch.tensor([pp['r'] if pp else 0 for pp in pps], dtype=torch.int32, device=dev),
+                    have=torch.tensor([pp is not None for pp in pps], dtype=torch.bool, device=dev))
 
     UTABLE_TOL = 5e-7        # max interpolation error of the tabulated radial coordinates relative to max|g| (float64, grid midpoints)
 
@@ -384,7 +392,7 @@ class ConvSE3(nn.Module):
         per edge.  Accepted only if the interpolant reproduces the float64 trunk at the grid MIDPOINTS to UTABLE_TOL (smooth
         radial functions pass by orders of magnitude; a rougher one falls back to se3_radial_trunk_u_fwd)."""
         Gn = grid.shape[0]
-        KT = max(16 * ((bases[p][0] + 1 + 15) // 16) for p in self.pairs)
+        KT = max(lowrank_k(bases[p][0]) for p in self.pairs)
         tab = torch.zeros((len(self.pairs), Gn, KT), dtype=torch.float32, device=dev)
         mid = (grid[:-1] + grid[1:]) * 0.5
         featm = self.encode_dist(mid)
@@ -441,12 +449,7 @@ class ConvSE3(nn.Module):
     # ---- forward ----------------------------------------------------------------------------------------
     def edge_features(self, edge_info, rel_dist):
         _, _, edges = edge_info
-        rd = rel_dist.unsqueeze(-1)
-        if self.fourier_encode_dist:
-            # reference utils.py:96-104: [sin(x / 2^s), cos(x / 2^s), x]
-            scales = 2 ** torch.arange(self.num_fourier_features, device=rd.device, dtype=rd.dtype)
-            xs = rd / scales
-            rd = torch.cat([xs.sin(), xs.cos(), rd], dim=-1)
+        rd = self.encode_dist(rel_dist.unsqueeze(-1))
         feat = torch.cat((rd, edges), dim=-1) if exists(edges) else rd
         return feat.reshape(-1, feat.shape[-1]).contiguous()
 
@@ -459,6 +462,11 @@ def input_side(di, do):
     The fused kernel then spends 2 l_in + 1 instead of 2 l_out + 1 FMAs per radial weight; worth it for l_in <= 1 < l_out
     and for l_in = 0 (measured: (0,3) 7.7 -> 2.6 ms, (1,3) 19.3 -> ~11.4 ms at cfg2 widths)."""
     return di < do and di <= 1 and not os.environ.get('SE3B200_NO_INPUT_SIDE')
+
+
+def lowrank_k(r):
+    """K of a rank-r low-rank pair: r columns of U and its ones column, padded to a multiple of 16."""
+    return 16 * ((r + 1 + 15) // 16)
 
 
 def use_zgemm():
@@ -545,16 +553,95 @@ class LowRankPlanMiss(RuntimeError):
     """The radial trunk outputs of a forward left the cached low-rank subspace (distances beyond the plan's range)."""
 
 
+def edge_chunks(E, tile_bytes):
+    """(t0, tile_count, e0, ec) of consecutive chunks of edge tiles such that a chunk's workspace (tile_bytes per tile of
+    ops.TILE_E edges) fits T_WORKSPACE_BYTES; edges e0 .. e0 + ec."""
+    n_tiles = (E + ops.TILE_E - 1) // ops.TILE_E
+    per_chunk = max(1, min(n_tiles, T_WORKSPACE_BYTES // tile_bytes))
+    for t0 in range(0, n_tiles, per_chunk):
+        tc = min(per_chunk, n_tiles - t0)
+        e0 = t0 * ops.TILE_E
+        yield t0, tc, e0, min(E - e0, tc * ops.TILE_E)
+
+
+class ConvDispatch:
+    """How one ConvSE3 runs in one forward (conv_dispatch).  route: 'production' (DESIGN.md 4.5, GEMM images z), 'aligned' (4.4)
+    or 'rfirst' (4.1-4.3, with each pair's kernel in how: 'input_side', 'combined', 'tc' or 'simt').  U [pairs, E, 64]: radial
+    coordinates of the low-rank pairs lr = {pair: plan entry}; g [pairs, E, 128]: trunk outputs for the direct kernels.  Outputs
+    go to outs {do: [E, Co, 2do+1]}, or on the production route to pooled or aligned_out."""
+
+    def __init__(self, conv, route, U, g, lr, z, how, outs):
+        self.conv, self.route, self.U, self.g, self.lr, self.z, self.how, self.outs = conv, route, U, g, lr, z, how, outs
+        self.pooled = self.self_out = None
+        self.aligned_out = {}
+
+
+def _forward_plan(conv, tc_ok, E, rel_dist, geom, capturing):
+    """The low-rank plan this forward of `conv` reads, or None (direct kernels)."""
+    pk = conv.packed()
+    if os.environ.get('SE3B200_NO_LOWRANK') or conv.edge_dim != 0:
+        return None
+    if conv.free_master and pk.get('lr') is not None:
+        return pk['lr']                     # built by pack_weights(max_distance=...) before the masters went away:
+                                            # the only image there is, whatever the edge count
+    if ops.lowrank_enabled(E) and any(tc_ok.values()) and not conv.free_master and not getattr(conv, '_lr_blocked', False):
+        if capturing:
+            return pk.get('lr')             # built by the warm-up forwards; the residual check still covers it
+        # cached; needs the distance range (one host sync per forward, in Geometry)
+        return conv.lowrank_plan(geom.d_max(rel_dist) if geom is not None else float(rel_dist.max()))
+    return None
+
+
+def conv_dispatch(conv, edge_info, rel_dist, geom, capturing):
+    """Choose the route of `conv` for this forward and launch its radial kernels (U of the low-rank pairs from the plan's table
+    or the trunk, g for the direct kernels).  The plan is checked here, or the check is queued on geom.deferred."""
+    idx = edge_info[0]
+    E, dev = idx.numel(), idx.device
+    pk = conv.packed()
+    feat = conv.edge_features(edge_info, rel_dist)
+    assert feat.shape[-1] == conv.in_dim, f'edge feature width {feat.shape[-1]} != {conv.in_dim}'
+    tc_ok = {pair: conv.tc_eligible(*pair) for pair in conv.pairs}
+    plan = _forward_plan(conv, tc_ok, E, rel_dist, geom, capturing)
+    lr, U, g, route = {}, None, None, 'rfirst'
+    if plan is not None and plan['pairs']:
+        covered = len(plan['pairs']) == len(conv.pairs)
+        stats = torch.zeros((len(conv.pairs), 2), dtype=torch.float32, device=dev)
+        if covered and plan['utab'] is not None and use_utable():
+            U = ops.radial_table(rel_dist, plan['utab'], plan['D'], plan['ones_col'], stats)
+        else:
+            U, g = ops.radial_trunk_u(feat, pk['trunk'], plan['Vstack'], plan['gmean'], plan['ones_col'], stats, want_g=not covered)
+        lr = dict(plan['pairs'])
+        check = (conv, stats, plan['have'])
+        if geom is not None and geom.deferred is not None:
+            geom.deferred.append(check)          # checked once per forward by the caller
+        elif check_lowrank_stats([check]):
+            # the fp32 trunk outputs of this forward leave the cached subspace (distances beyond the plan's range)
+            if conv.free_master:
+                raise LowRankPlanMiss('low-rank radial plan does not cover this input; pack_weights(max_distance=...) was given too '
+                                      'small a distance')
+            lr = {}                              # evaluate this ConvSE3 with the direct K = 128 kernels
+    kinds = {pp['kind'] for pp in lr.values()}
+    if kinds & {'z', 'aligned'}:                 # edge-aligned plans cover every pair of the ConvSE3 and need the Geometry
+        if geom is None:
+            raise RuntimeError('ConvSE3 was called with a (flat, plan) basis: the edge-aligned low-rank plan needs the third element, '
+                               'model.Geometry(rel_pos, max_degree), as SE3Transformer.forward passes it (or set SE3B200_NO_ALIGNED=1)')
+        route = 'production' if 'z' in kinds else 'aligned'
+    elif len(lr) < len(conv.pairs) and g is None:
+        g = ops.radial_trunk(feat, pk['trunk'], len(conv.pairs))       # the direct kernels consume g itself
+    how = {pair: lr[pair]['kind'] if pair in lr else 'tc' if tc_ok[pair] else 'simt' for pair in conv.pairs}
+    outs = {do: torch.empty((E, mo, to_order(do)), dtype=torch.float32, device=dev) for do, mo in conv.fiber_out}
+    return ConvDispatch(conv, route, U, g, lr, plan['z'] if route == 'production' else None, how, outs)
+
+
 def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False):
     """Evaluate one or more ConvSE3 that share input features, graph and fibers (to_k / to_v of an attention block)
     in a single sweep: the T blocks (gather x basis) are built once per (degree pair, edge chunk) and consumed by every
-    convolution's fused pairwise kernel."""
+    convolution's fused pairwise kernel.  conv_dispatch chooses each convolution's route; the production convolutions run
+    first, then the edge-aligned ones, then the R-first ones (the last two share one T workspace)."""
     c0 = convs[0]
     forward_only_guard('ConvSE3', convs, list(inp.values()) + [rel_dist])
-    idx, nmask, _ = edge_info
-    b, n, k = idx.shape
-    E = b * n * k
-    dev = idx.device
+    idx = edge_info[0]
+    E = idx.numel()
     if isinstance(basis, dict):
         raise TypeError("ConvSE3 takes the basis as the tuple (flat buffer, BasisPlan, Geometry) that SE3Transformer.forward builds: "
                         "`ops.basis_flat(rel_pos, max_degree) + (model.Geometry(rel_pos, max_degree),)`; the dict returned by the "
@@ -562,158 +649,98 @@ def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False):
     flat, plan = basis[:2]                   # BasisFlat (+ Geometry)
     geom = basis[2] if len(basis) > 2 else None
     bpairs = ops.basis_pairs(flat, plan, E)
-    n_tiles = (E + ops.TILE_E - 1) // ops.TILE_E
-
-    states = []
     capturing = torch.cuda.is_current_stream_capturing()
+    states = []
     for conv in convs:
         assert conv.pairs == c0.pairs and conv.in_dim == c0.in_dim
-        pk = conv.packed()
-        feat = conv.edge_features(edge_info, rel_dist)
-        assert feat.shape[-1] == conv.in_dim, f'edge feature width {feat.shape[-1]} != {conv.in_dim}'
-        tc_ok = {pair: conv.tc_eligible(*pair) for pair in conv.pairs}
-        # low-rank radial path (distance-only radial functions): U = G V with the pair's cached basis, K = r+1 <= 64
-        lr, lr_plan = {}, None
-        if os.environ.get('SE3B200_NO_LOWRANK') or conv.edge_dim != 0:
-            pass
-        elif conv.free_master and pk.get('lr') is not None:
-            lr_plan = pk['lr']                      # built by pack_weights(max_distance=...) before the masters went away:
-                                                    # the only image there is, whatever the edge count
-        elif ops.lowrank_enabled(E) and any(tc_ok.values()) and not conv.free_master and not getattr(conv, '_lr_blocked', False):
-            if capturing:
-                lr_plan = pk.get('lr')              # built by the warm-up forwards; the residual check below still covers it
-            else:                                   # cached; needs the distance range (one host sync per forward, in Geometry)
-                lr_plan = conv.lowrank_plan(geom.d_max(rel_dist) if geom is not None else float(rel_dist.max()))
-        g, U, zplan = None, None, None
-        if lr_plan is not None and lr_plan['pairs']:
-            if 'Vstack' not in lr_plan:
-                Vs = torch.zeros((len(conv.pairs), ops.RADIAL_MID, 64), dtype=torch.float32, device=dev)
-                gm = torch.zeros((len(conv.pairs), ops.RADIAL_MID), dtype=torch.float32, device=dev)
-                ones_col = torch.zeros(len(conv.pairs), dtype=torch.int32, device=dev)
-                have = torch.zeros(len(conv.pairs), dtype=torch.bool, device=dev)
-                for pi, pair in enumerate(conv.pairs):
-                    pp = lr_plan['pairs'].get(pair)
-                    if pp is not None:
-                        Vs[pi] = pp['V']
-                        gm[pi] = pp['gmean']
-                        ones_col[pi] = pp['r']
-                        have[pi] = True
-                lr_plan['Vstack'], lr_plan['gmean'], lr_plan['ones_col'], lr_plan['have'] = Vs, gm, ones_col, have
-            # trunk + U = G V + the residual statistics of the cached subspace on THIS forward's edges, one kernel
-            covered = len(lr_plan['pairs']) == len(conv.pairs)
-            stats = torch.zeros((len(conv.pairs), 2), dtype=torch.float32, device=dev)
-            if covered and lr_plan.get('utab') is not None and use_utable():
-                # distance-only radial functions: U(d) interpolated from the plan's float64 table; the guard is the table's range
-                U, g = ops.radial_table(rel_dist, lr_plan['utab'], lr_plan['D'], lr_plan['ones_col'], stats), None
-            else:
-                U, g = ops.radial_trunk_u(feat, pk['trunk'], lr_plan['Vstack'], lr_plan['gmean'], lr_plan['ones_col'], stats, want_g=not covered)
-            for pi, pair in enumerate(conv.pairs):
-                pp = lr_plan['pairs'].get(pair)
-                if pp is not None:
-                    lr[pair] = dict(Kp=pp['Kp'], U=U[pi], img=pp['img'], imgs_f=pp.get('imgs_f'), al_imgs=pp.get('al_imgs'))
-            check = (conv, stats, lr_plan['have'])
-            if geom is not None and geom.deferred is not None:
-                geom.deferred.append(check)          # checked once per forward by the caller
-            elif check_lowrank_stats([check]):
-                # the fp32 trunk outputs of this forward leave the cached subspace (distances beyond the plan's range)
-                if conv.free_master:
-                    raise LowRankPlanMiss('low-rank radial plan does not cover this input; pack_weights(max_distance=...) was given too '
-                                          'small a distance')
-                lr = {}                              # evaluate this ConvSE3 with the direct K = 128 kernel
-            if lr and covered and geom is not None:
-                zplan = lr_plan.get('z')
-        outs = {do: torch.empty((E, mo, to_order(do)), dtype=torch.float32, device=dev) for do, mo in conv.fiber_out}
-        al = zplan is None and geom is not None and len(lr) == len(conv.pairs) and all(v.get('al_imgs') is not None for v in lr.values())
-        if zplan is None and not al and any(v.get('img') is None and v.get('imgs_f') is None for v in lr.values()):
-            # the plan holds edge-aligned images only (DESIGN.md 4.4-4.5); they need the per-forward Geometry
-            if geom is None:
-                raise RuntimeError('ConvSE3 was called with a (flat, plan) basis: the edge-aligned low-rank plan needs the third element, '
-                                   'model.Geometry(rel_pos, max_degree), as SE3Transformer.forward passes it (or set SE3B200_NO_ALIGNED=1)')
-            lr = {}                                  # mixed eligibility inside one ConvSE3: direct kernels for this forward
-        if zplan is None and len(lr) < len(conv.pairs) and g is None:
-            g = ops.radial_trunk(feat, pk['trunk'], len(conv.pairs))       # the direct kernels consume g itself
-        states.append(dict(conv=conv, pk=pk, g=g, U=U, outs=outs, use_tc=tc_ok, lr=lr, aligned=al, z=zplan, lr_plan=lr_plan))
-    states_z_and_rest = list(states)            # in the order of `convs`
-    z_states = [st for st in states if st['z'] is not None]
-    states = [st for st in states if st['z'] is None]
-    if z_states:
-        # ---- production path (DESIGN.md 4.5): neighbour features rotated into the edge frame once per input degree, then ONE
-        # tensor-core GEMM per (conv, degree_out, |m|) over all input degrees, then the rotation back to the global frame
-        frames = geom.frames()
-        sx = ops.edge_scale(inp, idx, max(di for di, _ in c0.fiber_in))
-        per_tile = sum(mi * to_order(di) for di, mi in c0.fiber_in) * ops.TILE_E * 4
-        tpc = max(1, min(n_tiles, T_WORKSPACE_BYTES // per_tile))
-        # pooled convolutions (conv_in / conv_out): masked mean over the neighbours + self-interaction fused into the rotate-back
-        # (needs edge chunks that hold whole neighbour lists)
-        fuse_pool = tpc >= n_tiles or (tpc * ops.TILE_E) % k == 0
-        for st in z_states:
-            conv = st['conv']
-            if conv.pool and fuse_pool:
-                st['pooled'] = {do: torch.empty((b * n, mo, to_order(do)), dtype=torch.float32, device=dev) for do, mo in conv.fiber_out}
-                st['self'] = conv.self_interact(inp) if conv.self_interaction else {}
-        nmask_flat = None if nmask is None else nmask.reshape(-1)
-        for st in z_states:
-            if keep_aligned and 'pooled' not in st:      # the consumer (attention) rotates back on the fly: keep out' itself
-                st['aligned_out'] = {do: torch.empty((E, to_order(do), mo), dtype=torch.float32, device=dev)
-                                     for do, mo in st['conv'].fiber_out if do > 0}
-        for t0 in range(0, n_tiles, tpc):
-            tc = min(tpc, n_tiles - t0)
-            e0 = t0 * ops.TILE_E
-            ec = min(E - e0, tc * ops.TILE_E)
-            X = {di: ops.rotgather(inp[str(di)], idx, frames.D[di] if di > 0 else None, t0, tc) for di, _ in c0.fiber_in}
-            for st in z_states:
-                conv = st['conv']
-                for do, mo in conv.fiber_out:
-                    P = to_order(do)
-                    full = all((do, m) in st['z'] for m in range(do + 1))
-                    if do == 0 and 'pooled' not in st:
-                        Op = st['outs'][0][e0:e0 + ec]                   # [ec, mo, 1] is [ec, 1, mo]
-                    elif do in st.get('aligned_out', {}):
-                        Op = st['aligned_out'][do][e0:e0 + ec]
-                        if not full:
-                            Op.zero_()
-                    else:
-                        Op = (torch.empty if full else torch.zeros)((ec, P, mo), dtype=torch.float32, device=dev)
-                    for m in range(do + 1):
-                        zp = st['z'].get((do, m))
-                        if zp is None:
-                            continue
-                        segs, alg = [], 0
-                        for di, mi in zp['degs']:
-                            pi = conv.pairs.index((di, do))
-                            for kc in range(st['lr'][(di, do)]['Kp'] // 16):
-                                segs.append((st['U'][pi, e0:e0 + ec, 16 * kc:], X[di], mi, to_order(di), di + m, di - m))
-                            alg += ec * mo * mi * 2 * (ops.RADIAL_MID + P) * (1 if m == 0 else 2)
-                        ops.zgemm(segs, zp['img'], sx[e0:e0 + ec], ec, mo, zp['mode'], Op, P * mo, [(do + m) * mo, (do - m) * mo],
-                                  alg_flops=alg, tag=f'mode{zp["mode"]}lo{do}m{m}Co{mo}S{zp["S"]}')
-                    if 'pooled' in st:                  # rotate back + masked mean over k + self-interaction, one kernel
-                        sa = st['self'].get(str(do))
-                        ops.rotate_pool(Op, frames.D[do][e0:e0 + ec] if do > 0 else None, None if nmask_flat is None else nmask_flat[e0:e0 + ec],
-                                        None if sa is None else sa.reshape(b * n, mo, P)[e0 // k:(e0 + ec) // k], ec // k, k, mo, do,
-                                        st['pooled'][do][e0 // k:(e0 + ec) // k])
-                    elif do in st.get('aligned_out', {}):
-                        pass                            # stays in the edge frame; rotated inside the attention kernel
-                    elif do > 0:                        # back to the global frame: out = D_lo out'
-                        ops.fold_basis(Op.view(1, ec, P, mo), frames.D[do][e0:e0 + ec].reshape(-1), ec, mo, P, P, 1,
-                                       st['outs'][do][e0:e0 + ec], accumulate=False, component_major=True, name='rotate_back')
-            del X
-    aligned_states = [st for st in states if st['aligned']]
-    states_all, states = states_z_and_rest, [st for st in states if not st['aligned']]
-
-    # chunk over edge tiles so that the largest T block fits the workspace
-    worst = max(ops.t_numel(1, mi, to_order(min(di, do)), to_order(do)) * 4
-                for di, mi in c0.fiber_in for do, _ in c0.fiber_out)
-    tiles_per_chunk = max(1, min(n_tiles, T_WORKSPACE_BYTES // worst))
+        states.append(conv_dispatch(conv, edge_info, rel_dist, geom, capturing))
+    routes = {r: [st for st in states if st.route == r] for r in ('production', 'aligned', 'rfirst')}
+    if routes['production']:
+        _production_forward(routes['production'], inp, edge_info, geom, keep_aligned)
+    # the R-first routes chunk over edge tiles so that the largest T block fits the workspace
+    t_bytes = max(ops.t_numel(1, mi, to_order(min(di, do)), to_order(do)) * 4 for di, mi in c0.fiber_in for do, _ in c0.fiber_out)
     workspace = None
-    for t0 in range(0, n_tiles, tiles_per_chunk) if aligned_states else ():
-        # ---- edge-aligned formulation: rotate the neighbour features into the edge frame, two output components per launch
-        tc = min(tiles_per_chunk, n_tiles - t0)
-        e0 = t0 * ops.TILE_E
-        ec = min(E - e0, tc * ops.TILE_E)
-        frames = geom.frames()
+    if routes['aligned']:
+        workspace = _aligned_forward(routes['aligned'], inp, idx, geom, t_bytes, workspace)
+    if routes['rfirst']:
+        _rfirst_forward(routes['rfirst'], inp, idx, bpairs, t_bytes, workspace)
+    return [_conv_results(st, inp, edge_info) for st in states]
+
+
+def _production_forward(states, inp, edge_info, geom, keep_aligned):
+    """DESIGN.md 4.5: the neighbour features rotated into the edge frame once per input degree and edge chunk, ONE GEMM per
+    (conv, degree_out, |m|) over all input degrees, then the rotation back: fused with the masked mean and the self-interaction
+    for pooled convolutions (conv_in / conv_out), or left to the attention kernel with keep_aligned."""
+    idx, nmask, _ = edge_info
+    b, n, k = idx.shape
+    fiber_in = states[0].conv.fiber_in
+    frames = geom.frames()
+    sx = ops.edge_scale(inp, idx, max(di for di, _ in fiber_in))
+    chunks = list(edge_chunks(idx.numel(), sum(mi * to_order(di) for di, mi in fiber_in) * ops.TILE_E * 4))
+    fuse_pool = all(e0 % k == 0 for _, _, e0, _ in chunks)      # the fused pool needs chunks of whole neighbour lists
+    for st in states:
+        conv = st.conv
+        if conv.pool and fuse_pool:
+            st.pooled = {do: torch.empty((b * n, mo, to_order(do)), dtype=torch.float32, device=idx.device) for do, mo in conv.fiber_out}
+            st.self_out = conv.self_interact(inp) if conv.self_interaction else {}
+        elif keep_aligned:                   # the consumer (attention) rotates back on the fly: keep out' itself
+            st.aligned_out = {do: torch.empty((idx.numel(), to_order(do), mo), dtype=torch.float32, device=idx.device)
+                              for do, mo in conv.fiber_out if do > 0}
+    nmask_flat = None if nmask is None else nmask.reshape(-1)
+    for t0, tc, e0, ec in chunks:
+        X = {di: ops.rotgather(inp[str(di)], idx, frames.D[di] if di > 0 else None, t0, tc) for di, _ in fiber_in}
+        for st in states:
+            for do, mo in st.conv.fiber_out:
+                P = to_order(do)
+                Op = _zgemm_degree(st, do, mo, X, sx, e0, ec)
+                if st.pooled is not None:        # rotate back + masked mean over k + self-interaction, one kernel
+                    sa = st.self_out.get(str(do))
+                    ops.rotate_pool(Op, frames.D[do][e0:e0 + ec] if do > 0 else None, None if nmask_flat is None else nmask_flat[e0:e0 + ec],
+                                    None if sa is None else sa.reshape(b * n, mo, P)[e0 // k:(e0 + ec) // k], ec // k, k, mo, do,
+                                    st.pooled[do][e0 // k:(e0 + ec) // k])
+                elif do > 0 and do not in st.aligned_out:        # back to the global frame: out = D_lo out'
+                    ops.fold_basis(Op.view(1, ec, P, mo), frames.D[do][e0:e0 + ec].reshape(-1), ec, mo, P, P, 1,
+                                   st.outs[do][e0:e0 + ec], accumulate=False, component_major=True, name='rotate_back')
+        del X
+
+
+def _zgemm_degree(st, do, mo, X, sx, e0, ec):
+    """out' [ec, 2do+1, Co] (edge frame, component major) of output degree do on edges e0 .. e0 + ec: one zgemm per |m|, whose
+    K segments are the 16-column blocks of U of every input degree."""
+    conv, P = st.conv, to_order(do)
+    full = all((do, m) in st.z for m in range(do + 1))
+    if do == 0 and st.pooled is None:
+        Op = st.outs[0][e0:e0 + ec]                   # [ec, mo, 1] is [ec, 1, mo]
+    elif do in st.aligned_out:
+        Op = st.aligned_out[do][e0:e0 + ec]
+        if not full:
+            Op.zero_()
+    else:
+        Op = (torch.empty if full else torch.zeros)((ec, P, mo), dtype=torch.float32, device=sx.device)
+    for m in range(do + 1):
+        zp = st.z.get((do, m))
+        if zp is None:
+            continue
+        segs, alg = [], 0
+        for di, mi in zp['degs']:
+            pi = conv.pairs.index((di, do))
+            for kc in range(st.lr[(di, do)]['Kp'] // 16):
+                segs.append((st.U[pi, e0:e0 + ec, 16 * kc:], X[di], mi, to_order(di), di + m, di - m))
+            alg += ec * mo * mi * 2 * (ops.RADIAL_MID + P) * (1 if m == 0 else 2)
+        ops.zgemm(segs, zp['img'], sx[e0:e0 + ec], ec, mo, zp['mode'], Op, P * mo, [(do + m) * mo, (do - m) * mo],
+                  alg_flops=alg, tag=f'mode{zp["mode"]}lo{do}m{m}Co{mo}S{zp["S"]}')
+    return Op
+
+
+def _aligned_forward(states, inp, idx, geom, t_bytes, workspace):
+    """DESIGN.md 4.4: per edge chunk and (input degree, |m|), the neighbour features rotated into the edge frame (T blocks of
+    the aligned basis), two output components per pairwise_lr launch, then the rotation back to the global frame."""
+    c0 = states[0].conv
+    frames = geom.frames()
+    for t0, tc, e0, ec in edge_chunks(idx.numel(), t_bytes):
         # out' of degree do lives in one dense buffer per |m|: [edges, C_out] for m = 0, [edges, C_out, 2] = (+m, -m) otherwise
         # (the kernel's native layout); first contribution overwrites, later input degrees accumulate
-        outp = [{} for _ in aligned_states]
+        outp = [{} for _ in states]
         for di, mi in c0.fiber_in:
             for m in range(di + 1):
                 targets = [(do, mo) for do, mo in c0.fiber_out if do >= m]
@@ -723,83 +750,86 @@ def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False):
                 workspace = ops.tbuild_blocks(inp[str(di)], idx, frames.block(di, m), Pk, Fk, t0, tc, out=workspace)
                 for do, mo in targets:
                     P = to_order(do)
-                    for st, op in zip(aligned_states, outp):
-                        lrp = st['lr'][(di, do)]
+                    for st, op in zip(states, outp):
+                        lrp = st.lr[(di, do)]
                         first = (do, m) not in op
                         if first:
-                            op[(do, m)] = st['outs'][do][e0:e0 + ec] if do == 0 else torch.empty((ec, mo, Pk), dtype=torch.float32, device=dev)
-                        ops.pairwise_lr(lrp['U'][e0:e0 + ec], lrp['al_imgs'][m], workspace, ec, mo, mi, Fk, Pk, lrp['Kp'], op[(do, m)],
-                                        accumulate=not first, alg_units=Fk * 2 * (ops.RADIAL_MID + P))
-        for st, op in zip(aligned_states, outp):
+                            op[(do, m)] = st.outs[do][e0:e0 + ec] if do == 0 else torch.empty((ec, mo, Pk), dtype=torch.float32, device=idx.device)
+                        ops.pairwise_lr(st.U[c0.pairs.index((di, do)), e0:e0 + ec], lrp['images'][m], workspace, ec, mo, mi, Fk, Pk,
+                                        lrp['Kp'], op[(do, m)], accumulate=not first, alg_units=Fk * 2 * (ops.RADIAL_MID + P))
+        for st, op in zip(states, outp):
             for do, mo in c0.fiber_out:
                 if do > 0:                      # back to the global frame: out = D_lo out'
                     ops.rotate_back([op.get((do, m)) for m in range(do + 1)], frames.D[do][e0:e0 + ec].reshape(-1), ec, mo, do,
-                                    st['outs'][do][e0:e0 + ec])
+                                    st.outs[do][e0:e0 + ec])
                 elif (0, 0) not in op:
-                    st['outs'][0][e0:e0 + ec].zero_()
+                    st.outs[0][e0:e0 + ec].zero_()
         del outp
-    for t0 in range(0, n_tiles, tiles_per_chunk) if states else ():
-        tc = min(tiles_per_chunk, n_tiles - t0)
-        e0 = t0 * ops.TILE_E
-        ec = min(E - e0, tc * ops.TILE_E)
+    return workspace
+
+
+def _rfirst_forward(states, inp, idx, bpairs, t_bytes, workspace):
+    """DESIGN.md 4.1-4.3 in the global frame: per edge chunk and degree pair one T block (gather x basis) shared by every
+    convolution, then per convolution the pair's kernel -- combined low-rank, direct tensor-core or SIMT -- accumulating over
+    the input degrees; or the input-side contraction, on the gathered neighbour features, folded with the basis afterwards."""
+    c0 = states[0].conv
+    for t0, tc, e0, ec in edge_chunks(idx.numel(), t_bytes):
         gathered = {}                            # degree_in -> neighbour features of this chunk in tile layout
         for do, mo in c0.fiber_out:
             P = to_order(do)
-            first = True
+            accumulate = False                   # the first input degree overwrites, the others accumulate
             for di, mi in c0.fiber_in:
-                Fq = to_order(min(di, do))
-                Q = to_order(di)
-                in_side = [input_side(di, do) and (di, do) in st['lr'] and st['lr'][(di, do)]['imgs_f'] is not None for st in states]
-                if any(in_side) and di not in gathered:
-                    gathered[di] = ops.gather_tiles(inp[str(di)], idx, t0, tc)
-                if not all(in_side):
-                    workspace = ops.tbuild(inp[str(di)], idx, bpairs[(di, do)], di, do, t0, tc, out=workspace)
+                Fq, Q = to_order(min(di, do)), to_order(di)
                 pi = c0.pairs.index((di, do))
-                for st, ins in zip(states, in_side):
-                    conv = st['conv']
-                    out = st['outs'][do][e0:e0 + ec]
-                    if ins:
+                hows = [st.how[(di, do)] for st in states]
+                if 'input_side' in hows and di not in gathered:
+                    gathered[di] = ops.gather_tiles(inp[str(di)], idx, t0, tc)
+                if any(h != 'input_side' for h in hows):
+                    workspace = ops.tbuild(inp[str(di)], idx, bpairs[(di, do)], di, do, t0, tc, out=workspace)
+                for st, how in zip(states, hows):
+                    conv = st.conv
+                    out = st.outs[do][e0:e0 + ec]
+                    if how == 'input_side':
                         # S[f,e,o,q] = sum_i R[e,o,i,f] x[j(e),i,q], then out[e,o,p] (+)= sum_{f,q} B[e,p,q,f] S[f,e,o,q]
-                        lrp = st['lr'][(di, do)]
-                        S = torch.empty((Fq, ec, mo, Q), dtype=torch.float32, device=dev)
+                        S = torch.empty((Fq, ec, mo, Q), dtype=torch.float32, device=idx.device)
                         for f in range(Fq):
-                            ops.pairwise_lr(lrp['U'][e0:e0 + ec], lrp['imgs_f'][f], gathered[di], ec, mo, mi, 1, Q, lrp['Kp'], S[f],
-                                            accumulate=False, alg_P=P)
+                            ops.pairwise_lr(st.U[pi, e0:e0 + ec], st.lr[(di, do)]['images'][f], gathered[di], ec, mo, mi, 1, Q,
+                                            st.lr[(di, do)]['Kp'], S[f], accumulate=False, alg_P=P)
                         ops.fold_basis(S, bpairs[(di, do)][e0 * P * Q * Fq:(e0 + ec) * P * Q * Fq], ec, mo, P, Q, Fq, out,
-                                       accumulate=not first)
+                                       accumulate=accumulate)
                         del S
-                    elif (di, do) in st['lr']:
-                        lrp = st['lr'][(di, do)]
-                        ops.pairwise_lr(lrp['U'][e0:e0 + ec], lrp['img'], workspace, ec, mo, mi, Fq, P, lrp['Kp'], out,
-                                        accumulate=not first)
-                    elif st['use_tc'][(di, do)]:
-                        ops.pairwise_tc(st['g'][pi, e0:e0 + ec], conv.w3_image(di, do), workspace, ec, mo, mi, Fq, P,
-                                        out, accumulate=not first)
+                    elif how == 'combined':
+                        ops.pairwise_lr(st.U[pi, e0:e0 + ec], st.lr[(di, do)]['images'][0], workspace, ec, mo, mi, Fq, P,
+                                        st.lr[(di, do)]['Kp'], out, accumulate=accumulate)
+                    elif how == 'tc':
+                        ops.pairwise_tc(st.g[pi, e0:e0 + ec], conv.w3_image(di, do), workspace, ec, mo, mi, Fq, P, out,
+                                        accumulate=accumulate)
                     else:
                         lin = conv.kernel_unary[f'({di},{do})'].rp.net['6']
-                        ops.pairwise_simt(st['g'][pi, e0:e0 + ec], lin.weight, lin.bias, workspace, ec, mo, mi, Fq, P, out,
-                                          accumulate=not first)
-                first = False
+                        ops.pairwise_simt(st.g[pi, e0:e0 + ec], lin.weight, lin.bias, workspace, ec, mo, mi, Fq, P, out,
+                                          accumulate=accumulate)
+                accumulate = True
+    return workspace
 
-    results = []
-    for st in states_all:
-        conv = st['conv']
-        outputs = {}
-        if 'pooled' in st:
-            results.append({str(do): st['pooled'][do].view(b, n, mo, to_order(do)) for do, mo in conv.fiber_out})
-            continue
-        for do, mo in conv.fiber_out:
-            if do in st.get('aligned_out', {}):
-                outputs[str(do)] = AlignedKV(st['aligned_out'][do].view(b, n, k, to_order(do), mo), do)
-                continue
-            o = st['outs'][do].view(b, n, k, mo, to_order(do))
-            if conv.pool:
-                o = ops.pool(o, nmask)
-            outputs[str(do)] = o
-        if conv.self_interaction:
-            outputs = residual_add(outputs, conv.self_interact(inp))
-        results.append(outputs)
-    return results
+
+def _conv_results(st, inp, edge_info):
+    """The outputs of one convolution as the reference returns them: pooled over the neighbours and with the self-interaction
+    added where the ConvSE3 asks for them; AlignedKV for degrees kept in the edge frame."""
+    conv = st.conv
+    idx, nmask, _ = edge_info
+    b, n, k = idx.shape
+    if st.pooled is not None:
+        return {str(do): st.pooled[do].view(b, n, mo, to_order(do)) for do, mo in conv.fiber_out}
+    outputs = {}
+    for do, mo in conv.fiber_out:
+        if do in st.aligned_out:
+            outputs[str(do)] = AlignedKV(st.aligned_out[do].view(b, n, k, to_order(do), mo), do)
+        else:
+            o = st.outs[do].view(b, n, k, mo, to_order(do))
+            outputs[str(do)] = ops.pool(o, nmask) if conv.pool else o
+    if conv.self_interaction:
+        outputs = residual_add(outputs, conv.self_interact(inp))
+    return outputs
 
 
 class FeedForwardSE3(nn.Module):

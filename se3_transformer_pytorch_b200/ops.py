@@ -353,26 +353,28 @@ def t_numel(num_tiles, Ci, F, P):
     return num_tiles * nifb * TILE_IF * ph * TILE_E * 4
 
 
-def tbuild(x, idx, basis_pair, d_in, d_out, tile_begin=0, tile_count=None, out=None):
-    """x [b,n,Ci,2di+1], idx [b,n,k], basis_pair flat [E*P*Q*F] -> T (tile layout, see include/se3b200.h)."""
-    _require_cuda(x, idx, basis_pair)
-    x = _f32(x)
-    b, n, Ci, Q = x.shape
-    k = idx.shape[-1]
-    P, F = 2 * d_out + 1, 2 * min(d_in, d_out) + 1
-    E = b * n * k
-    n_tiles = (E + TILE_E - 1) // TILE_E
+def _tile_range(E, tile_begin, tile_count):
+    """(tile_count, edges) of a launch over tiles tile_begin .. tile_begin + tile_count of E edges (None: to the last tile)."""
     if tile_count is None:
-        tile_count = n_tiles - tile_begin
+        tile_count = (E + TILE_E - 1) // TILE_E - tile_begin
+    return tile_count, min(E - tile_begin * TILE_E, tile_count * TILE_E)
+
+
+def _tbuild_launch(x, idx, blocks, P, F, tile_begin, tile_count, out, flops, nbytes):
+    """se3_tbuild_fwd into `out` (reallocated if missing or too small): x [b,n,Ci,Q] fp32, blocks [E,P,Q,F] flat."""
+    b, n, Ci, Q = x.shape
     numel = t_numel(tile_count, Ci, F, P)
     if out is None or out.numel() < numel:
         out = torch.empty(numel, dtype=torch.float32, device=x.device)
-    Ec = min(E - tile_begin * TILE_E, tile_count * TILE_E)       # edges of this call; bytes WITHOUT the layout padding of T
-    nbytes = 4 * Ec * (Ci * F * P + P * Q * F + Ci * Q) + 8 * Ec
-    with torch.cuda.device(x.device), _timed('tbuild', flops=2 * Ec * Ci * F * P * Q, nbytes=nbytes):
-        _check(lib().se3_tbuild_fwd(_p(x), _p(idx.contiguous()), _p(basis_pair), b, n, k, Ci, P, Q, F, tile_begin, tile_count,
+    with torch.cuda.device(x.device), _timed('tbuild', flops=flops, nbytes=nbytes):
+        _check(lib().se3_tbuild_fwd(_p(x), _p(idx.contiguous()), _p(blocks), b, n, idx.shape[-1], Ci, P, Q, F, tile_begin, tile_count,
                                     _p(out), _stream()))
     return out
+
+
+def tbuild(x, idx, basis_pair, d_in, d_out, tile_begin=0, tile_count=None, out=None):
+    """x [b,n,Ci,2di+1], idx [b,n,k], basis_pair flat [E*P*Q*F] -> T (tile layout, see include/se3b200.h)."""
+    return tbuild_blocks(x, idx, basis_pair, 2 * d_out + 1, 2 * min(d_in, d_out) + 1, tile_begin, tile_count, out)
 
 
 _IDENTITY_BASIS = {}
@@ -384,24 +386,14 @@ def gather_tiles(x, idx, tile_begin=0, tile_count=None, out=None):
     _require_cuda(x, idx)
     x = _f32(x)
     b, n, Ci, Q = x.shape
-    k = idx.shape[-1]
-    E = b * n * k
+    E = b * n * idx.shape[-1]
     key = (E, Q, x.device)
     if key not in _IDENTITY_BASIS:
         _IDENTITY_BASIS.clear()
         _IDENTITY_BASIS[key] = torch.eye(Q, dtype=torch.float32, device=x.device).repeat(E, 1, 1).reshape(-1).contiguous()
-    eye = _IDENTITY_BASIS[key]
-    n_tiles = (E + TILE_E - 1) // TILE_E
-    if tile_count is None:
-        tile_count = n_tiles - tile_begin
-    numel = t_numel(tile_count, Ci, 1, Q)
-    if out is None or out.numel() < numel:
-        out = torch.empty(numel, dtype=torch.float32, device=x.device)
-    Ec = min(E - tile_begin * TILE_E, tile_count * TILE_E)
-    nbytes = 4 * Ec * (2 * Ci * Q) + 8 * Ec
-    with torch.cuda.device(x.device), _timed('tbuild', flops=2 * Ec * Ci * Q * Q, nbytes=nbytes):
-        _check(lib().se3_tbuild_fwd(_p(x), _p(idx.contiguous()), _p(eye), b, n, k, Ci, Q, Q, 1, tile_begin, tile_count, _p(out), _stream()))
-    return out
+    tile_count, Ec = _tile_range(E, tile_begin, tile_count)
+    return _tbuild_launch(x, idx, _IDENTITY_BASIS[key], Q, 1, tile_begin, tile_count, out, flops=2 * Ec * Ci * Q * Q,
+                          nbytes=4 * Ec * (2 * Ci * Q) + 8 * Ec)
 
 
 def tbuild_blocks(x, idx, blocks, P, F, tile_begin=0, tile_count=None, out=None):
@@ -409,20 +401,12 @@ def tbuild_blocks(x, idx, blocks, P, F, tile_begin=0, tile_count=None, out=None)
     _require_cuda(x, idx, blocks)
     x = _f32(x)
     b, n, Ci, Q = x.shape
-    k = idx.shape[-1]
-    E = b * n * k
+    E = b * n * idx.shape[-1]
     assert blocks.numel() == E * P * Q * F
-    n_tiles = (E + TILE_E - 1) // TILE_E
-    if tile_count is None:
-        tile_count = n_tiles - tile_begin
-    numel = t_numel(tile_count, Ci, F, P)
-    if out is None or out.numel() < numel:
-        out = torch.empty(numel, dtype=torch.float32, device=x.device)
-    Ec = min(E - tile_begin * TILE_E, tile_count * TILE_E)
-    nbytes = 4 * Ec * (Ci * F * P + P * Q * F + Ci * Q) + 8 * Ec
-    with torch.cuda.device(x.device), _timed('tbuild', flops=2 * Ec * Ci * F * P * Q, nbytes=nbytes):
-        _check(lib().se3_tbuild_fwd(_p(x), _p(idx.contiguous()), _p(blocks), b, n, k, Ci, P, Q, F, tile_begin, tile_count, _p(out), _stream()))
-    return out
+    tile_count, Ec = _tile_range(E, tile_begin, tile_count)
+    # bytes WITHOUT the layout padding of T
+    return _tbuild_launch(x, idx, blocks, P, F, tile_begin, tile_count, out, flops=2 * Ec * Ci * F * P * Q,
+                          nbytes=4 * Ec * (Ci * F * P + P * Q * F + Ci * Q) + 8 * Ec)
 
 
 def fold_basis(S, basis_pair, E, Co, P, Q, F, out, accumulate, component_major=False, name='fold_basis'):
@@ -493,7 +477,7 @@ def pack_lowrank(Fp, Co, Ci, F, Kp):
     return img
 
 
-def pairwise_lr(U, w_img, T, E, Co, Ci, F, P, Kp, out, accumulate, alg_P=None, out_strides=None, p_off=None, alg_units=None):
+def pairwise_lr(U, w_img, T, E, Co, Ci, F, P, Kp, out, accumulate, alg_P=None, alg_units=None):
     """Low-rank radial path: U [E,64] fp32 (G V | 1 | 0), w_img from pack_lowrank."""
     _require_cuda(U, w_img, T, out)
     # algorithmic work of the reference formulation (SURVEY.md 8d): 2*128 (radial GEMM) + 2P (contraction) per R element;
@@ -508,12 +492,7 @@ def pairwise_lr(U, w_img, T, E, Co, Ci, F, P, Kp, out, accumulate, alg_P=None, o
     tag = f'P{P}F{F}Ci{Ci}Co{Co}K{Kp}' + (f'(in-side of P{alg_P})' if alg_P is not None else '')
     with torch.cuda.device(out.device), _timed('pairwise_lr', flops=flops, nbytes=nbytes, tag=tag,
                                                mma=2 * E * Co * Ci * F * 3 * Kp, fma=2 * E * Co * Ci * F * P):
-        if out_strides is None:
-            _check(lib().se3_pairwise_lr_fwd(_p(U), _p(w_img), _p(T), E, Co, Ci, F, P, Kp, int(accumulate), _p(out), _stream()))
-        else:
-            offs = (ctypes.c_int * P)(*p_off)
-            _check(lib().se3_pairwise_lr_strided_fwd(_p(U), _p(w_img), _p(T), E, Co, Ci, F, P, Kp, int(accumulate), _p(out),
-                                                     out_strides[0], out_strides[1], offs, _stream()))
+        _check(lib().se3_pairwise_lr_fwd(_p(U), _p(w_img), _p(T), E, Co, Ci, F, P, Kp, int(accumulate), _p(out), _stream()))
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -594,14 +573,10 @@ def rotgather(x, idx, D, tile_begin=0, tile_count=None, out=None):
     x = _f32(x)
     b, n, Ci, Q = x.shape
     k = idx.shape[-1]
-    E = b * n * k
-    n_tiles = (E + TILE_E - 1) // TILE_E
-    if tile_count is None:
-        tile_count = n_tiles - tile_begin
+    tile_count, Ec = _tile_range(b * n * k, tile_begin, tile_count)
     numel = tile_count * Ci * Q * TILE_E
     if out is None or out.numel() < numel:
         out = torch.empty(numel, dtype=torch.float32, device=x.device)
-    Ec = min(E - tile_begin * TILE_E, tile_count * TILE_E)
     nbytes = 4 * Ec * (2 * Ci * Q + (Q * Q if Q > 1 else 0)) + 8 * Ec
     with torch.cuda.device(x.device), _timed('rotgather', flops=2 * Ec * Ci * Q * Q, nbytes=nbytes):
         _check(lib().se3_rotgather_fwd(_p(x), _p(idx.contiguous()), _p(D), b, n, k, Ci, Q, tile_begin, tile_count, _p(out), _stream()))

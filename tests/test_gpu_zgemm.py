@@ -70,7 +70,7 @@ def _run_zgemm(mode, Co, E, seg_shapes, flush=0, seed=0, x_scale=1.0, positive=F
 
 
 @pytest.mark.parametrize('mode,Co,E,segs', [
-    (1, 256, 300, [(8, 1, 0, 0, 16)]),                                     # N = 256, 3 edge tiles (padding CTA in the 2-cluster)
+    (1, 256, 300, [(8, 1, 0, 0, 16)]),                                     # N = 256, 3 edge tiles (the last one partly filled)
     (1, 128, 128, [(4, 3, 1, 1, 16), (12, 5, 2, 2, 16)]),                  # N = 128 tile, two input degrees
     (1, 512, 257, [(16, 1, 0, 0, 16), (8, 3, 1, 1, 32), (4, 7, 3, 3, 16)]),  # a K = 32 pair (two sub-segments)
     (2, 128, 300, [(6, 3, 2, 0, 16)]),                                     # (+m, -m) = components 2, 0 of an l = 1 input
@@ -80,20 +80,15 @@ def _run_zgemm(mode, Co, E, seg_shapes, flush=0, seed=0, x_scale=1.0, positive=F
     (3, 256, 200, [(4, 3, 2, 0, 16), (12, 5, 3, 1, 32), (4, 7, 4, 2, 16)]),
     (3, 512, 129, [(32, 7, 6, 0, 16)]),
 ])
-@pytest.mark.parametrize('pair', [0, 3])
-def test_zgemm_matches_fp64(mode, Co, E, segs, pair, monkeypatch):
-    """pair = 3: the cta_group::2 variant (one MMA of the leader CTA drives both SMs of the cluster, each CTA streams half of the
-    weights; an option, off by default -- see se3_zgemm_fwd)."""
+@pytest.mark.parametrize('flush', [0, 1, 2, 3, 7])
+def test_zgemm_matches_fp64(mode, Co, E, segs, flush):
+    """One launch against float64, with the fp32 drain of the accumulators every `flush` stages (0: the default schedule)."""
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, Co, 1):
         pytest.skip('needs sm_90')
-    if pair and mode == 2:
-        pytest.skip('pair mode exists for modes 1 and 3')
-    monkeypatch.setenv('SE3B200_Z_PAIR', str(pair))
-    for flush in (0, 1, 2, 3, 7):
-        out, ref = _run_zgemm(mode, Co, E, segs, flush=flush, seed=flush)
-        err = rel_err(out.cpu().numpy(), ref.cpu().numpy())
-        assert err < (6e-6 if mode == 3 else 3e-6), f'flush={flush}: {err:.3e}'
+    out, ref = _run_zgemm(mode, Co, E, segs, flush=flush, seed=flush)
+    err = rel_err(out.cpu().numpy(), ref.cpu().numpy())
+    assert err < (6e-6 if mode == 3 else 3e-6), f'flush={flush}: {err:.3e}'
 
 
 @pytest.mark.parametrize('x_scale', [1e-6, 1.0, 3e4])
