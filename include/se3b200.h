@@ -13,7 +13,7 @@
  *                                                                                               se3_pairwise_{simt,tc}_fwd
  *   masked_mean pooling of ConvSE3                     utils.py:72-80, S:256-257             -> se3_pool_fwd
  *   AttentionSE3.forward logits/softmax/aggregate      se3_transformer_pytorch.py:476-517    -> se3_attn_fwd
- *     (low-rank radial path: se3_pack_lowrank + se3_pairwise_lr_fwd / _strided_fwd, se3_fold_basis_fwd, se3_rotate_back_fwd:
+ *     (low-rank radial path: se3_pack_lowrank + se3_pairwise_lr_fwd, se3_fold_basis_fwd, se3_rotate_back_fwd:
  *      the same product re-associated; DESIGN.md 4.2-4.4)
  *   NormSE3.forward (next to the hot path, SURVEY 8f)  se3_transformer_pytorch.py:130-152    -> se3_norm_fwd
  *
@@ -44,7 +44,7 @@ extern "C" {
 #define SE3_TILE_IF        4  /* (in-channel, frequency) pairs per tile step */
 
 const char* se3_last_error(void);
-int         se3_abi_version(void);
+int         se3_abi_version(void);     /* 2; raised with every incompatible change of the entry points below */
 
 /* Neighbour graph (S:1171-1294).  For every node i of every cloud: the k smallest "modified" distances over the
  * other n-1 nodes, ascending (ties: lower node index first), exactly as the reference's remove-self + topk:
@@ -129,13 +129,6 @@ int se3_pack_lowrank(const float* Fp, int Co, int Ci, int F, int Kp, void* image
 int se3_pairwise_lr_fwd(const float* U, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F, int P,
                         int Kp, int accumulate, float* out, void* stream);
 
-/* As se3_pairwise_lr_fwd, but component p of the kernel is written to out[e*edge_stride + o*channel_stride + p_off[p]]
- * (p_off: HOST array of P ints, P in {1,2,3,5,7}).  Used by the edge-aligned formulation (DESIGN.md 4.4), where one launch
- * updates the components (+m, -m) of a component-major [E, P_full, Co] buffer (channel_stride = 1). */
-int se3_pairwise_lr_strided_fwd(const float* U, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F, int P,
-                                int Kp, int accumulate, float* out, int64_t edge_stride, int channel_stride, const int* p_off,
-                                void* stream);
-
 /* Basis fold of the input-side contraction (pairs with 2 l_in + 1 = Q < P = 2 l_out + 1; S:336-343, 251 reassociated):
  *   out[e,o,p] (+)= sum_{f,q} basis_pair[e,p,q,f] * S[f,e,o,q]
  * where S[f] [E,Co,Q] = se3_pairwise_lr_fwd with F := 1, P := Q, T := the gathered neighbour features in tile layout
@@ -209,7 +202,7 @@ typedef struct se3_zseg {
  *   mode 3 (|m| > 0):  the same two planes with three real products per complex one (Gauss): S1 = sum (a+b) c, S2 = sum a (d-c),
  *                      S3 = sum b (c+d), c = x'[cplus], d = x'[cminus]; plane + = S1 - S3, plane - = S1 + S2  (3/4 of mode 2's work)
  * on the Hopper tensor cores, Z generated on the fly into wgmma operand registers (3-pass fp16 split, fp32 partial sums drained every
- * flush_stages (0 = default) stages of 64 K values).  w_img: se3_zgemm_pack of every segment in order.  Co % 128 == 0,
+ * flush_stages (0 = the default: 24 for mode 3, 8 otherwise) stages of 64 K values).  w_img: se3_zgemm_pack of every segment in order.  Co % 128 == 0,
  * (Ci * F) % 4 == 0 (F = 1 for mode 1, else 2; mode 3: Ci % 4 == 0), <= 16 segments (HOST array).  out rows: edge stride out_edge_stride floats, plane c at comp_off{c}. */
 int     se3_zgemm_tile_n(int Co, int mode);
 int64_t se3_zgemm_image_bytes(int Co, int mode, int total_stages);
@@ -240,9 +233,10 @@ int se3_attn_fwd(const float* q, const float* k, const float* v, const int64_t* 
  * out / res [nodes, Eo, M] in the reference layout (no transposed copies), 3-pass fp16 split with fp32 partial sums as in
  * se3_zgemm_fwd.  w_img = se3_zgemm_pack(Fp = W^T [Eo, D] viewed as [Eo * D/16, 16], Kp 16, col0 0, Co Eo, CiF D/16, mode 4,
  * total_stages D/64, stage0 0) (se3_zgemm_image_bytes(Eo, 4, D/64) bytes).  sx [nodes]: se3_pow2_scale_fwd of the row maxima
- * (se3_rowabsmax_fwd) with target exponent 14.  D % 64 == 0, Eo % 128 == 0.  res may be NULL. */
+ * (se3_rowabsmax_fwd) with target exponent 14.  D % 64 == 0, Eo % 128 == 0.  res may be NULL.  The fp32 partial sums are drained
+ * every flush_stages stages (0 = the default, 8). */
 int se3_linear_tc_fwd(const float* x, const void* w_img, const float* res, const float* sx, int64_t nodes, int D, int Eo, int M,
-                      float* out, void* stream);
+                      float* out, int flush_stages, void* stream);
 /* sx[r] = power of two with rowmax[r] * sx[r] in [2^(target_exp-1), 2^target_exp) (1 for zero / non-finite rows). */
 int se3_pow2_scale_fwd(const float* rowmax, int64_t rows, int target_exp, float* sx, void* stream);
 

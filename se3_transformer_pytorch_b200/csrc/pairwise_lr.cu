@@ -68,13 +68,12 @@ extern "C" int se3_pack_lowrank(const float* Fp, int Co, int Ci, int F, int Kp, 
   return SE3_OK;
 }
 
-static int pairwise_lr_impl(const float* U, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F, int P, int Kp,
-                            int accumulate, float* out, int64_t out_es, int out_os, const int* p_off, void* stream) {
+extern "C" int se3_pairwise_lr_fwd(const float* U, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F, int P,
+                                   int Kp, int accumulate, float* out, void* stream) {
   using namespace se3;
   SE3_REQUIRE(E > 0 && Co > 0 && Ci > 0 && F > 0, "se3_pairwise_lr_fwd: bad sizes");
   SE3_REQUIRE(Co % SE3_TILE_O == 0, "se3_pairwise_lr_fwd: Co=%d must be a multiple of %d", Co, SE3_TILE_O);
   SE3_REQUIRE(P == 1 || P == 2 || P == 3 || P == 5 || P == 7, "se3_pairwise_lr_fwd: P=%d unsupported (1, 2, 3, 5, 7)", P);
-  SE3_REQUIRE(out_es > 0 && out_os > 0, "se3_pairwise_lr_fwd: bad output strides");
   SE3_REQUIRE(Kp >= 16 && Kp <= 64 && Kp % 16 == 0, "se3_pairwise_lr_fwd: Kp=%d must be 16, 32, 48 or 64", Kp);
   SE3_REQUIRE(ceil_div(E, SE3_TILE_E) * (Co / SE3_TILE_O) < 2147483647ll, "se3_pairwise_lr_fwd: grid too large");
   PwParams prm = {};
@@ -89,11 +88,9 @@ static int pairwise_lr_impl(const float* U, const void* w_img, const float* T, i
   prm.n_ob = Co / SE3_TILE_O;
   prm.accumulate = accumulate;
   prm.nk16 = Kp / 16;
-  prm.out_es = out_es;
-  prm.out_os = out_os;
-  for (int p = 0; p < 7; ++p) prm.p_off[p] = (p < P) ? (p_off ? p_off[p] : p) : 0;
-  for (int p = 0; p < P; ++p)
-    SE3_REQUIRE(prm.p_off[p] >= 0 && prm.p_off[p] < out_es, "se3_pairwise_lr_fwd: p_off[%d]=%d outside the edge row", p, prm.p_off[p]);
+  prm.out_es = (int64_t)Co * P;
+  prm.out_os = P;
+  for (int p = 0; p < 7; ++p) prm.p_off[p] = p;
   prm.spu = lr_steps_per_unit(Kp);
   prm.NU = (int)ceil_div((int64_t)prm.NIFB, (int64_t)prm.spu);
   cudaStream_t s = as_stream(stream);
@@ -104,18 +101,4 @@ static int pairwise_lr_impl(const float* U, const void* w_img, const float* T, i
     case 5: return launch_pw<5, false, false, 4>(prm, s);
     default: return launch_pw<7, false, false, 4>(prm, s);
   }
-}
-
-extern "C" int se3_pairwise_lr_fwd(const float* U, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F, int P,
-                                   int Kp, int accumulate, float* out, void* stream) {
-  return pairwise_lr_impl(U, w_img, T, E, Co, Ci, F, P, Kp, accumulate, out, (int64_t)Co * P, P, nullptr, stream);
-}
-
-// As se3_pairwise_lr_fwd, writing component p of the kernel to out[e*edge_stride + o*channel_stride + p_off[p]] (p_off: HOST
-// array of P ints): the edge-aligned formulation (DESIGN.md 4.4) updates two components (+m, -m) of a component-major
-// [E, P_full, Co] buffer per launch (channel_stride 1: every thread writes 8 consecutive floats per component).
-extern "C" int se3_pairwise_lr_strided_fwd(const float* U, const void* w_img, const float* T, int64_t E, int Co, int Ci, int F,
-                                           int P, int Kp, int accumulate, float* out, int64_t edge_stride, int channel_stride,
-                                           const int* p_off, void* stream) {
-  return pairwise_lr_impl(U, w_img, T, E, Co, Ci, F, P, Kp, accumulate, out, edge_stride, channel_stride, p_off, stream);
 }

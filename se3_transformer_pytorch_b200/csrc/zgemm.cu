@@ -477,11 +477,6 @@ static int launch_z(const ZParams& prm, cudaStream_t s) {
   return SE3_OK;
 }
 
-static int z_env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return v ? atoi(v) : dflt;
-}
-
 }  // namespace se3
 
 extern "C" int se3_zgemm_tile_n(int Co, int mode) {
@@ -517,9 +512,9 @@ extern "C" int se3_zgemm_pack(const float* Fp, int Kp, int col0, int Co, int CiF
 // LinearSE3 on the tensor cores (reference S:78-95): out[node, o, m] = sum_d x[node, d, m] W[d, o] (+ res[node, o, m]) with the A
 // operand read in place from the reference layout (row = (node, m), stride M), split to fp16 hi / lo on the fly; the same
 // pipeline as se3_zgemm_fwd (MODE 4: one N = 128 accumulator, fp32 drain).  w_img = se3_zgemm_pack(W^T viewed [Eo * D/16, 16],
-// Kp 16, col0 0, Co Eo, CiF D/16, mode 4).  sx [nodes]: power-of-two scale per node (se3_node_scale_fwd).
+// Kp 16, col0 0, Co Eo, CiF D/16, mode 4).  sx [nodes]: power-of-two scale per node (se3_pow2_scale_fwd).
 extern "C" int se3_linear_tc_fwd(const float* x, const void* w_img, const float* res, const float* sx, int64_t nodes, int D, int Eo,
-                                 int M, float* out, void* stream) {
+                                 int M, float* out, int flush_stages, void* stream) {
   using namespace se3;
   SE3_REQUIRE(nodes > 0 && M >= 1 && M <= 11, "se3_linear_tc_fwd: bad sizes");
   SE3_REQUIRE(D > 0 && D % 64 == 0 && Eo > 0 && Eo % 128 == 0, "se3_linear_tc_fwd: D=%d must be a multiple of 64 and Eo=%d of 128", D, Eo);
@@ -542,7 +537,7 @@ extern "C" int se3_linear_tc_fwd(const float* x, const void* w_img, const float*
   prm.n_mt = (int)ceil_div(prm.E, SE3_TILE_E);
   prm.n_nt = Eo / 128;
   prm.S = D / 64;
-  prm.flush_stages = std::max(1, z_env_int("SE3B200_Z_FLUSH", 8));
+  prm.flush_stages = flush_stages > 0 ? flush_stages : 8;
   return launch_z<4, 128, 128>(prm, as_stream(stream));
 }
 
@@ -586,8 +581,7 @@ extern "C" int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img,
   prm.S = S;
   // default drain period: 96 accumulating K = 16 MMAs per accumulator (8 stages of 12; mode 3 spreads its stages over three
   // accumulators): rel. error 4e-6 against float64 for all-positive operands at K = 65536 (2.5e-4 if never drained)
-  prm.flush_stages = std::max(1, flush_stages > 0 ? flush_stages
-                                                     : z_env_int("SE3B200_Z_FLUSH", mode == 3 ? 24 : 8) * std::max(1, z_env_int("SE3B200_Z_FLUSH_MULT", 1)));
+  prm.flush_stages = flush_stages > 0 ? flush_stages : (mode == 3 ? 24 : 8);
   cudaStream_t s = as_stream(stream);
   if (mode == 3) return launch_z<3, 128, 64>(prm, s);
   if (mode == 2) return launch_z<2, 128, 64>(prm, s);

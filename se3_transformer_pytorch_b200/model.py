@@ -9,14 +9,13 @@ libse3b200.so through `ops`; the cheap glue around it (embeddings, LinearSE3 GEM
 Forward only: everything runs under torch.no_grad().  CUDA only: there is no CPU fallback.
 """
 import operator
-import os
 from math import sqrt
 
 import torch
 import torch.nn.functional as F
 from torch import nn
 
-from . import ops
+from . import ops, switches
 from . import aligned as _aligned
 
 
@@ -105,14 +104,16 @@ class LinearSE3(nn.Module):
         return hit[1]
 
     def forward(self, x, residual=None):
+        sw = switches.current()
+        tc = not (sw.force_simt or sw.no_linear_tc)
         out = {}
         for degree, w in self.weights.items():
             t = x[degree]                                            # [b, n, d, m]
             res = residual.get(degree) if residual is not None else None
-            if t.is_cuda and t.dtype == torch.float32 and not torch.is_grad_enabled() and ops.linear_supported(w.shape[0], w.shape[1], t.device):
+            if tc and t.is_cuda and t.dtype == torch.float32 and not torch.is_grad_enabled() and ops.linear_supported(w.shape[0], w.shape[1], t.device):
                 img = self.image(degree)
                 if img is not None:
-                    out[degree] = ops.linear_tc(t, img, w.shape[1], res=res)
+                    out[degree] = ops.linear_tc(t, img, w.shape[1], res=res, flush_stages=sw.linear_flush())
                     continue
             y = torch.matmul(t.transpose(-1, -2), w).transpose(-1, -2).contiguous()
             out[degree] = y if res is None else y + res
@@ -228,32 +229,47 @@ class ConvSE3(nn.Module):
             self.self_interact = LinearSE3(fiber_in, fiber_out)
         self._packed = None
         self.free_master = False
+        self._lr_blocked = False      # set when a forward left the low-rank plan: the direct kernels from then on
+        self.utable_error = None      # interpolation error of the last radial table built (radial_table)
 
     # ---- packed weights ---------------------------------------------------------------------------------
     def _param_version(self):
-        v = []
-        for p in self.kernel_unary.parameters():
-            v.append((p._version, p.data_ptr()))
-        return tuple(v)
+        return tuple((p._version, p.data_ptr()) for p in self.kernel_unary.parameters())
 
-    def packed(self):
-        """Trunk parameter pack [pairs, stride] (built lazily, rebuilt when weights change) + a cache of the tensor-core
-        images of net.6 for the direct (K = 128) kernel, filled on demand by w3_image()."""
+    # the switches the low-rank plan reads (it is built from tc_eligible, which reads force_simt)
+    PLAN_SWITCHES = ('force_simt', 'no_aligned', 'no_zgemm', 'z_mode2', 'no_input_side', 'no_utable', 'lowrank_tol')
+
+    def _weights(self):
+        """What depends on the weights alone, built lazily and rebuilt when they change: the trunk parameter pack [pairs, stride]
+        and the tensor-core images of net.6 for the direct (K = 128) kernel, filled on demand by w3_image()."""
         ver = None if self.free_master else self._param_version()
-        if self._packed is not None and (self.free_master or self._packed['version'] == ver):
-            return self._packed
-        with torch.no_grad():
-            trunk = torch.stack([self.kernel_unary[f'({di},{do})'].rp.trunk_params() for di, do in self.pairs]).contiguous()
-        self._packed = dict(version=ver, trunk=trunk, images={}, tc_ok={})
+        if self._packed is None or not (self.free_master or self._packed['version'] == ver):
+            with torch.no_grad():
+                trunk = torch.stack([self.kernel_unary[f'({di},{do})'].rp.trunk_params() for di, do in self.pairs]).contiguous()
+            self._packed = dict(version=ver, trunk=trunk, images={}, tc_ok={}, tc_key=None, lr=None, lr_key=None)
         return self._packed
 
+    def packed(self, sw=None):
+        """_weights() with the decisions tc_ok {pair: tc_eligible} and lr (lowrank_plan), each dropped when a switch it reads has
+        changed in sw (default: switches.current()).  With released masters those of pack_weights stay, whatever the switches."""
+        pk = self._weights()
+        if not self.free_master:
+            sw = switches.current() if sw is None else sw
+            if pk['tc_key'] != sw.force_simt:
+                pk.update(tc_key=sw.force_simt, tc_ok={})
+            plan_key = tuple(getattr(sw, f) for f in self.PLAN_SWITCHES)
+            if pk['lr_key'] != plan_key:
+                pk.update(lr_key=plan_key, lr=None)
+        return pk
+
     def tc_eligible(self, di, do):
-        """The tensor-core kernels take this pair: sm_90, C_out % 32 == 0, degree_out <= 3 and operands inside the fp16 range
-        of the hi/lo split (|g| <= sqrt(127) max|ln.w| + max|ln.b| after LayerNorm + GELU)."""
-        pk = self.packed()
+        """The tensor-core kernels take this pair: not force_simt, sm_90, C_out % 32 == 0, degree_out <= 3 and operands inside
+        the fp16 range of the hi/lo split (|g| <= sqrt(127) max|ln.w| + max|ln.b| after LayerNorm + GELU)."""
+        sw = switches.current()
+        pk = self.packed(sw)
         if (di, do) not in pk['tc_ok']:
             pc = self.kernel_unary[f'({di},{do})']
-            ok = ops.tc_supported(pk['trunk'].device, pc.nc_out, pc.d_out)
+            ok = not sw.force_simt and ops.tc_supported(pk['trunk'].device, pc.nc_out, pc.d_out)
             if ok and (di, do) not in pk['images']:
                 lin, ln = pc.rp.net['6'], pc.rp.net['4']
                 g_bound = 11.3 * float(ln.weight.abs().max()) + float(ln.bias.abs().max())
@@ -262,7 +278,7 @@ class ConvSE3(nn.Module):
         return pk['tc_ok'][(di, do)]
 
     def w3_image(self, di, do):
-        pk = self.packed()
+        pk = self._weights()
         if (di, do) not in pk['images']:
             pc = self.kernel_unary[f'({di},{do})']
             lin = pc.rp.net['6']
@@ -286,27 +302,28 @@ class ConvSE3(nn.Module):
         xs = rd / scales
         return torch.cat([xs.sin(), xs.cos(), rd], dim=-1)
 
-    def lowrank_plan(self, d_max):
+    def lowrank_plan(self, d_max, sw=None):
         """Per pair: orthonormal V [128, r] spanning the curve g(d), d in [0, D], and the tensor-core images of F'' = [W3 V | b3 | 0]
         in the pair's formulation `kind`: if every pair has a plan, 'z' (in the per-(degree_out, |m|) GEMM images plan['z'],
         DESIGN.md 4.5) or 'aligned' (one image per |m|, 4.4); otherwise 'input_side' (one image per frequency, 4.3) or 'combined'
-        (4.2).  Depends on the weights and on D only: built once (and again if weights change or a forward brings a larger
-        distance).  Only for distance-only radial functions (no extra edge features)."""
-        pk = self.packed()
-        plan = pk.get('lr')
+        (4.2).  Depends on the weights, D and the PLAN_SWITCHES of sw (default: switches.current()): built once, and again if one
+        of them changes or a forward brings a larger distance.  Only for distance-only radial functions (no extra edge features)."""
+        sw = switches.current() if sw is None else sw
+        pk = self.packed(sw)
+        plan = pk['lr']
         if plan is not None and plan['D'] >= d_max:
             return plan
         dev = pk['trunk'].device
         D = 1.25 * d_max
         with torch.no_grad():
             grid = torch.linspace(0.0, D, self.LR_GRID, device=dev, dtype=torch.float64).unsqueeze(-1)
-            bases, ugrid = self._factor_curves(self.encode_dist(grid))
+            bases, ugrid = self._factor_curves(self.encode_dist(grid), sw.lowrank_tol)
             complete = len(bases) == len(self.pairs)
-            aligned = use_aligned() and complete
-            z = aligned and use_zgemm() and self.zgemm_eligible({pair: lowrank_k(rv[0]) for pair, rv in bases.items()})
+            aligned = not sw.no_aligned and complete
+            z = aligned and not sw.no_zgemm and self.zgemm_eligible({pair: lowrank_k(rv[0]) for pair, rv in bases.items()})
             pairs, zweights = {}, {}
             for pair, (r, V, gmean) in bases.items():
-                kind = 'z' if z else 'aligned' if aligned else 'input_side' if input_side(*pair) else 'combined'
+                kind = 'z' if z else 'aligned' if aligned else 'input_side' if not sw.no_input_side and input_side(*pair) else 'combined'
                 lin = self.kernel_unary[f'({pair[0]},{pair[1]})'].rp.net['6']
                 Fp = torch.zeros((lin.weight.shape[0], lowrank_k(r)), dtype=torch.float32, device=dev)
                 Fp[:, :r] = (lin.weight.double() @ V).float()
@@ -317,21 +334,21 @@ class ConvSE3(nn.Module):
                 Vp[:, :r] = V.float()
                 pairs[pair] = dict(kind=kind, r=r, Kp=Fp.shape[1], V=Vp, gmean=gmean.float(),
                                    images=[] if kind == 'z' else self._pack_images(pair, kind, Fp))
-            zplan = self._zgemm_images(zweights) if z else None
-            utab = self.radial_table(ugrid, bases, grid, dev) if complete and use_utable() else None
+            zplan = self._zgemm_images(zweights, 2 if sw.z_mode2 else 3) if z else None
+            utab = self.radial_table(ugrid, bases, grid, dev) if complete and not sw.no_utable else None
             plan = dict(D=D, pairs=pairs, z=zplan, utab=utab, **self._plan_stacks(pairs, dev))
         pk['lr'] = plan
         return plan
 
-    def _factor_curves(self, feat):
+    def _factor_curves(self, feat, tol):
         """Every tc-eligible pair that still has its net.6 weights and whose curve g(d) (float64 trunk on the distance grid
-        `feat`) has a low-rank model: {pair: (r, V, gmean)} and {pair: (U(d) = (g - gmean) V on the grid, max|g|)}."""
+        `feat`) has a low-rank model within tol: {pair: (r, V, gmean)} and {pair: (U(d) = (g - gmean) V on the grid, max|g|)}."""
         bases, ugrid = {}, {}
         for di, do in self.pairs:
             pc = self.kernel_unary[f'({di},{do})']
             if self.tc_eligible(di, do) and pc.rp.net['6'].weight.numel() > 0:
                 G64 = pc.rp.trunk64(feat)
-                basis = ops.lowrank_basis(G64)
+                basis = ops.lowrank_basis(G64, tol)
                 if basis is not None:
                     bases[(di, do)] = basis
                     ugrid[(di, do)] = ((G64 - basis[2]) @ basis[1], float(G64.abs().max()))
@@ -362,15 +379,16 @@ class ConvSE3(nn.Module):
             return [ops.pack_lowrank(Fv[:, :, f, :].reshape(-1, Kp).contiguous(), Co, Ci, 1, Kp) for f in range(nf)]
         return [ops.pack_lowrank(Fp, Co, Ci, nf, Kp)]
 
-    def _zgemm_images(self, zweights):
-        """{(do, m): dict(img, S, degs, mode)}: the aligned weights of the pairs (di >= m, do) as one GEMM image (DESIGN.md 4.5)."""
+    def _zgemm_images(self, zweights, mode_m):
+        """{(do, m): dict(img, S, degs, mode)}: the aligned weights of the pairs (di >= m, do) as one GEMM image (DESIGN.md 4.5);
+        the |m| > 0 images in kernel mode mode_m (3: three real products per complex one, 3/4 of the tensor-core work of 2)."""
         zplan = {}
         for do, mo in self.fiber_out:
             for m in range(do + 1):
                 degs = [(di, mi) for di, mi in self.fiber_in if di >= m]
                 if not degs:
                     continue
-                mode = 1 if m == 0 else z_mode_m()
+                mode = 1 if m == 0 else mode_m
                 img, S = ops.zgemm_image([(zweights[(di, do)][m], mi) for di, mi in degs], mo, mode)
                 zplan[(do, m)] = dict(img=img, S=S, degs=degs, mode=mode)
         return zplan
@@ -432,14 +450,15 @@ class ConvSE3(nn.Module):
         will see) and distance-only radial functions, the low-rank plan is built and pairs it covers need no direct
         (K = 128) image.  free_master=True then releases the fp32 net.6 weights of every imaged pair (inference only:
         state_dict() no longer holds them)."""
+        sw = switches.current()
         covered = {}
-        if max_distance is not None and self.edge_dim == 0 and not os.environ.get('SE3B200_NO_LOWRANK'):
-            covered = self.lowrank_plan(float(max_distance) / 1.25)['pairs']
+        if max_distance is not None and self.edge_dim == 0 and not sw.no_lowrank:
+            covered = self.lowrank_plan(float(max_distance) / 1.25, sw)['pairs']
         for di, do in self.pairs:
             if self.tc_eligible(di, do) and (di, do) not in covered:
                 self.w3_image(di, do)
         if free_master:
-            pk = self.packed()
+            pk = self._weights()
             self.free_master = True
             for key in list(pk['images']) + list(covered):
                 lin = self.kernel_unary[f'({key[0]},{key[1]})'].rp.net['6']
@@ -460,8 +479,8 @@ class ConvSE3(nn.Module):
 def input_side(di, do):
     """Degree pairs evaluated with the input-side contraction on the low-rank path: out = B . (R x) instead of R (B x).
     The fused kernel then spends 2 l_in + 1 instead of 2 l_out + 1 FMAs per radial weight; worth it for l_in <= 1 < l_out
-    and for l_in = 0 (measured: (0,3) 7.7 -> 2.6 ms, (1,3) 19.3 -> ~11.4 ms at cfg2 widths)."""
-    return di < do and di <= 1 and not os.environ.get('SE3B200_NO_INPUT_SIDE')
+    and for l_in = 0 (measured: (0,3) 7.7 -> 2.6 ms, (1,3) 19.3 -> ~11.4 ms at cfg2 widths).  Off with the no_input_side switch."""
+    return di < do and di <= 1
 
 
 def lowrank_k(r):
@@ -469,31 +488,13 @@ def lowrank_k(r):
     return 16 * ((r + 1 + 15) // 16)
 
 
-def use_zgemm():
-    """One GEMM per (degree_out, |m|) with the A operand generated on the fly (DESIGN.md 4.5) instead of the R-first kernels."""
-    return not os.environ.get('SE3B200_NO_ZGEMM')
-
-
-def use_utable():
-    """Radial coordinates by table lookup (se3_radial_table_fwd) instead of the per-edge radial MLP (se3_radial_trunk_u_fwd)."""
-    return not os.environ.get('SE3B200_NO_UTABLE')
-
-
-def z_mode_m():
-    """Kernel mode of the |m| > 0 launches: 3 = three real products per complex one (Gauss; 3/4 of the tensor-core work of mode 2)."""
-    return 2 if os.environ.get('SE3B200_Z_MODE2') else 3
-
-
-def use_aligned():
-    """Edge-aligned evaluation of the low-rank path (DESIGN.md 4.4): 2 FMAs per radial weight instead of 2 l_out + 1."""
-    return not os.environ.get('SE3B200_NO_ALIGNED')
-
-
 class Geometry:
-    """Per-forward edge geometry shared by every layer; the aligned frames are built on first use."""
+    """Per-forward edge geometry shared by every layer; the aligned frames are built on first use, by the code that the
+    host_frames switch selects when the Geometry is made."""
 
     def __init__(self, rel_pos, max_degree):
         self.rel_pos, self.max_degree, self._frames = rel_pos, max_degree, None
+        self.host_frames = switches.current().host_frames
         # run-time checks of the low-rank plans, as (ConvSE3, stats [pairs, 2]) : None = check inside every ConvSE3 (one host
         # synchronisation each); a list = the caller collects them and checks once per forward (SE3Transformer.forward)
         self.deferred = None
@@ -516,10 +517,10 @@ class Geometry:
         return out.view(b, n, k, C, P)
 
     def frames(self):
-        """Per-edge Wigner matrices D_l(R_e) (se3_frames_fwd, float64 arithmetic on the device; SE3B200_HOST_FRAMES=1: the
-        float64 torch restatement in aligned.py)."""
+        """Per-edge Wigner matrices D_l(R_e) (se3_frames_fwd, float64 arithmetic on the device; host_frames: the float64 torch
+        restatement in aligned.py)."""
         if self._frames is None:
-            if os.environ.get('SE3B200_HOST_FRAMES'):
+            if self.host_frames:
                 self._frames = _aligned.EdgeFrames(self.rel_pos, self.max_degree)
             else:
                 self._frames = _aligned.EdgeFrames(self.rel_pos, self.max_degree, D=ops.frames(self.rel_pos, self.max_degree))
@@ -568,27 +569,27 @@ class ConvDispatch:
     """How one ConvSE3 runs in one forward (conv_dispatch).  route: 'production' (DESIGN.md 4.5, GEMM images z), 'aligned' (4.4)
     or 'rfirst' (4.1-4.3, with each pair's kernel in how: 'input_side', 'combined', 'tc' or 'simt').  U [pairs, E, 64]: radial
     coordinates of the low-rank pairs lr = {pair: plan entry}; g [pairs, E, 128]: trunk outputs for the direct kernels.  Outputs
-    go to outs {do: [E, Co, 2do+1]}, or on the production route to pooled or aligned_out."""
+    go to outs {do: [E, Co, 2do+1]}, or on the production route to pooled or aligned_out.  sw: the switches of this forward."""
 
-    def __init__(self, conv, route, U, g, lr, z, how, outs):
-        self.conv, self.route, self.U, self.g, self.lr, self.z, self.how, self.outs = conv, route, U, g, lr, z, how, outs
+    def __init__(self, conv, sw, route, U, g, lr, z, how, outs):
+        self.conv, self.sw, self.route, self.U, self.g, self.lr, self.z, self.how, self.outs = conv, sw, route, U, g, lr, z, how, outs
         self.pooled = self.self_out = None
         self.aligned_out = {}
 
 
-def _forward_plan(conv, tc_ok, E, rel_dist, geom, capturing):
+def _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing):
     """The low-rank plan this forward of `conv` reads, or None (direct kernels)."""
-    pk = conv.packed()
-    if os.environ.get('SE3B200_NO_LOWRANK') or conv.edge_dim != 0:
+    pk = conv.packed(sw)
+    if sw.no_lowrank or conv.edge_dim != 0:
         return None
-    if conv.free_master and pk.get('lr') is not None:
+    if conv.free_master and pk['lr'] is not None:
         return pk['lr']                     # built by pack_weights(max_distance=...) before the masters went away:
                                             # the only image there is, whatever the edge count
-    if ops.lowrank_enabled(E) and any(tc_ok.values()) and not conv.free_master and not getattr(conv, '_lr_blocked', False):
+    if ops.lowrank_enabled(E, sw) and any(tc_ok.values()) and not conv.free_master and not conv._lr_blocked:
         if capturing:
-            return pk.get('lr')             # built by the warm-up forwards; the residual check still covers it
+            return pk['lr']                 # built by the warm-up forwards; the residual check still covers it
         # cached; needs the distance range (one host sync per forward, in Geometry)
-        return conv.lowrank_plan(geom.d_max(rel_dist) if geom is not None else float(rel_dist.max()))
+        return conv.lowrank_plan(geom.d_max(rel_dist) if geom is not None else float(rel_dist.max()), sw)
     return None
 
 
@@ -597,16 +598,17 @@ def conv_dispatch(conv, edge_info, rel_dist, geom, capturing):
     or the trunk, g for the direct kernels).  The plan is checked here, or the check is queued on geom.deferred."""
     idx = edge_info[0]
     E, dev = idx.numel(), idx.device
-    pk = conv.packed()
+    sw = switches.current()
+    pk = conv.packed(sw)
     feat = conv.edge_features(edge_info, rel_dist)
     assert feat.shape[-1] == conv.in_dim, f'edge feature width {feat.shape[-1]} != {conv.in_dim}'
     tc_ok = {pair: conv.tc_eligible(*pair) for pair in conv.pairs}
-    plan = _forward_plan(conv, tc_ok, E, rel_dist, geom, capturing)
+    plan = _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing)
     lr, U, g, route = {}, None, None, 'rfirst'
     if plan is not None and plan['pairs']:
         covered = len(plan['pairs']) == len(conv.pairs)
         stats = torch.zeros((len(conv.pairs), 2), dtype=torch.float32, device=dev)
-        if covered and plan['utab'] is not None and use_utable():
+        if covered and plan['utab'] is not None and not sw.no_utable:
             U = ops.radial_table(rel_dist, plan['utab'], plan['D'], plan['ones_col'], stats)
         else:
             U, g = ops.radial_trunk_u(feat, pk['trunk'], plan['Vstack'], plan['gmean'], plan['ones_col'], stats, want_g=not covered)
@@ -630,7 +632,7 @@ def conv_dispatch(conv, edge_info, rel_dist, geom, capturing):
         g = ops.radial_trunk(feat, pk['trunk'], len(conv.pairs))       # the direct kernels consume g itself
     how = {pair: lr[pair]['kind'] if pair in lr else 'tc' if tc_ok[pair] else 'simt' for pair in conv.pairs}
     outs = {do: torch.empty((E, mo, to_order(do)), dtype=torch.float32, device=dev) for do, mo in conv.fiber_out}
-    return ConvDispatch(conv, route, U, g, lr, plan['z'] if route == 'production' else None, how, outs)
+    return ConvDispatch(conv, sw, route, U, g, lr, plan['z'] if route == 'production' else None, how, outs)
 
 
 def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False):
@@ -728,7 +730,7 @@ def _zgemm_degree(st, do, mo, X, sx, e0, ec):
                 segs.append((st.U[pi, e0:e0 + ec, 16 * kc:], X[di], mi, to_order(di), di + m, di - m))
             alg += ec * mo * mi * 2 * (ops.RADIAL_MID + P) * (1 if m == 0 else 2)
         ops.zgemm(segs, zp['img'], sx[e0:e0 + ec], ec, mo, zp['mode'], Op, P * mo, [(do + m) * mo, (do - m) * mo],
-                  alg_flops=alg, tag=f'mode{zp["mode"]}lo{do}m{m}Co{mo}S{zp["S"]}')
+                  flush_stages=st.sw.zgemm_flush(zp['mode']), alg_flops=alg, tag=f'mode{zp["mode"]}lo{do}m{m}Co{mo}S{zp["S"]}')
     return Op
 
 
@@ -910,7 +912,7 @@ class AttentionSE3(nn.Module):
         queries = self.to_q(features)
         k_idx = None
         geom = basis[2] if isinstance(basis, tuple) and len(basis) > 2 else None
-        fuse = geom is not None and not os.environ.get('SE3B200_NO_ATTN_ROTATE')    # rotate-back fused into the attention kernel
+        fuse = geom is not None and not switches.current().no_attn_rotate    # rotate-back fused into the attention kernel
         if self.linear_proj_keys:
             values = conv_forward([self.to_v], features, edge_info, rel_dist, basis, keep_aligned=fuse)[0]
             keys = self.to_k(features)            # node level; the attention kernel gathers through idx
@@ -1479,7 +1481,8 @@ class SE3Transformer(nn.Module):
 class GraphedForward:
     """CUDA-graph replay of SE3Transformer.forward for fixed shapes.  Inputs are copied into static device buffers
     (host tensors are accepted: the copy is then the H2D transfer); the returned tensors are the graph's static outputs
-    and are overwritten by the next call."""
+    and are overwritten by the next call.  A replay runs the kernels the switches (switches.py) selected at capture; changing a
+    switch needs a new capture."""
 
     def __init__(self, model, feats, coors, mask=None, warmup=2, **fwd_kwargs):
         assert not model.attend_sparse_neighbors and fwd_kwargs.get('neighbor_mask') is None, \

@@ -36,7 +36,6 @@ _SIGNATURES = {
     'se3_lowrank_image_bytes': (c_int64, [c_int, c_int, c_int, c_int]),
     'se3_pack_lowrank': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_pairwise_lr_fwd': (c_int, [c_void_p] * 3 + [c_int64] + [c_int] * 6 + [c_void_p, c_void_p]),
-    'se3_pairwise_lr_strided_fwd': (c_int, [c_void_p] * 3 + [c_int64] + [c_int] * 6 + [c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     'se3_fold_basis_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_fold_basis_cm_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_rotate_back_fwd': (c_int, [c_void_p] * 5 + [c_int64, c_int, c_int, c_void_p, c_void_p]),
@@ -45,7 +44,7 @@ _SIGNATURES = {
     'se3_frames_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5),
     'se3_rotgather_fwd': (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_int64, c_int64, c_void_p, c_void_p]),
     'se3_rotate_pool_fwd': (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_int, c_void_p, c_void_p]),
-    'se3_linear_tc_fwd': (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_int, c_void_p, c_void_p]),
+    'se3_linear_tc_fwd': (c_int, [c_void_p] * 4 + [c_int64, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     'se3_pow2_scale_fwd': (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     'se3_rowabsmax_fwd': (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),
     'se3_edge_scale_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
@@ -611,8 +610,6 @@ def edge_scale(feats, idx, max_degree):
 
 def linear_supported(D, Eo, device):
     """Shapes the tensor-core LinearSE3 kernel takes."""
-    if os.environ.get('SE3B200_NO_LINEAR_TC') or os.environ.get('SE3B200_FORCE_SIMT'):
-        return False
     return D % 64 == 0 and Eo % 128 == 0 and torch.cuda.get_device_capability(device) == (9, 0)
 
 
@@ -630,8 +627,9 @@ def linear_image(W):
     return img
 
 
-def linear_tc(x, img, Eo, res=None):
-    """LinearSE3 on the tensor cores: x [b,n,D,M] (reference layout, read in place) -> [b,n,Eo,M] (+ res)."""
+def linear_tc(x, img, Eo, res=None, flush_stages=0):
+    """LinearSE3 on the tensor cores: x [b,n,D,M] (reference layout, read in place) -> [b,n,Eo,M] (+ res); the fp32 partial
+    sums are drained every flush_stages stages (0: the library's default)."""
     _require_cuda(x, img, res)
     x = _f32(x)
     b, n, D, M = x.shape
@@ -647,7 +645,7 @@ def linear_tc(x, img, Eo, res=None):
         _check(lib().se3_pow2_scale_fwd(_p(rowmax), nodes, 14, _p(sx), _stream()))
         nbytes = img.numel() + 4 * (2 * x.numel() + out.numel() * (2 if res is not None else 1))
         with _timed('linear', flops=2 * nodes * M * D * Eo, nbytes=nbytes, mma=2 * nodes * M * D * Eo * 3, tag=f'linear D{D}E{Eo}M{M}'):
-            _check(lib().se3_linear_tc_fwd(_p(x), _p(img), _p(res), _p(sx), nodes, D, Eo, M, _p(out), _stream()))
+            _check(lib().se3_linear_tc_fwd(_p(x), _p(img), _p(res), _p(sx), nodes, D, Eo, M, _p(out), flush_stages, _stream()))
     return out
 
 
@@ -708,15 +706,13 @@ def zgemm(segs, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off, flush_st
 LOWRANK_TOL = 1e-6
 
 
-def lowrank_basis(G64, tol=None, ranks=(15, 31, 47, 63)):
+def lowrank_basis(G64, tol=LOWRANK_TOL, ranks=(15, 31, 47, 63)):
     """Affine low-rank model of the curve G64 [S, 128] (float64 samples of a radial trunk along its input curve):
     returns (r, V [128, r] float64 orthonormal, mean [128] float64) for the smallest listed rank with
     max|(G - mean) - ((G - mean) V) V^T| <= tol * max|G|, else None.  The mean costs nothing downstream: W3 mean joins the bias
     column of F' (the ones column of U), and centring lowers the rank the tolerance needs by one (measured on 120 random
     trunks: ranks 14/15/16/17 for 26/52/22/1 % without, 13/14/15/16 with), so that ~99 % instead of ~78 % of the pairs fit K = 16.
     QR + SVD of the triangular factor (no Gram matrix, so the small singular directions stay accurate)."""
-    if tol is None:
-        tol = float(os.environ.get('SE3B200_LOWRANK_TOL', LOWRANK_TOL))
     G64 = G64.detach()
     mean = G64.mean(dim=0)
     H = G64 - mean
@@ -733,16 +729,16 @@ def lowrank_basis(G64, tol=None, ranks=(15, 31, 47, 63)):
     return None
 
 
-def lowrank_enabled(E):
-    if os.environ.get('SE3B200_NO_LOWRANK'):
-        return False
-    return E >= int(os.environ.get('SE3B200_LOWRANK_MIN_EDGES', 16384))
+def lowrank_enabled(E, sw=None):
+    """A forward of E edges takes the low-rank radial path under the switches sw (default: switches.current())."""
+    if sw is None:
+        from .switches import current
+        sw = current()
+    return not sw.no_lowrank and E >= sw.lowrank_min_edges
 
 
 def tc_supported(device, Co, P):
     """The wgmma kernel needs sm_90 and Co % 32 == 0, degree_out <= 3."""
-    if os.environ.get('SE3B200_FORCE_SIMT'):
-        return False
     if Co % TILE_O != 0 or P > 7:
         return False
     return torch.cuda.get_device_capability(device) == (9, 0)

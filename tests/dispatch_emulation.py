@@ -7,7 +7,6 @@ order they were packed in and their shape.  No CUDA is needed: tc_supported skip
 packed trunk parameters.
 """
 import contextlib
-import os
 
 import torch
 import torch.nn.functional as F
@@ -56,10 +55,12 @@ class Emulation:
     def __init__(self):
         self.trace = []
         self.labels = {}            # id(image) -> label
+        self.images = []            # the labelled images, kept alive so that their ids are not reused
 
     def _label(self, img, kind, desc):
         label = f'{kind}#{len(self.labels)}[{desc}]'
         self.labels[id(img)] = label
+        self.images.append(img)
         return label
 
     def _arg(self, v):
@@ -98,7 +99,7 @@ class Emulation:
         return img, S
 
     def tc_supported(self, device, Co, P):
-        return not os.environ.get('SE3B200_FORCE_SIMT') and Co % ops.TILE_O == 0 and P <= 7
+        return Co % ops.TILE_O == 0 and P <= 7
 
     # ---- radial functions -------------------------------------------------------------------------------
     def radial_trunk(self, feat, params, num_pairs):

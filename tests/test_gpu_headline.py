@@ -66,6 +66,18 @@ def _capture_attention(model, feats, coors, mask):
     return out, rec
 
 
+def _forward_simt(model, feats, coors, mask):
+    """The model's output with the force_simt switch on, and the kernel kinds that forward launched."""
+    from se3_transformer_pytorch_b200 import ops, switches
+    ops.PROFILE = []
+    try:
+        with switches.override(force_simt=True):
+            out = model(feats, coors, mask)
+    finally:
+        prof, ops.PROFILE = ops.PROFILE, None
+    return out, {p[0] for p in prof}
+
+
 def _oracle_block(rec, P_attn, nodes, nd, dim, heads, dim_head):
     """Oracle K, V, attention output (before to_out) of the sampled query nodes from the recorded block input."""
     idx, nmask, rel_pos, rel_dist = (t.cpu().numpy() for t in rec['graph'])
@@ -141,20 +153,13 @@ def test_production_path_matches_simt_whole_model():
         prof, ops.PROFILE = ops.PROFILE, None
     kinds = {p[0] for p in prof}
     assert kinds & {'zgemm', 'pairwise_lr'} and 'rotgather' in kinds, kinds
-    os.environ['SE3B200_FORCE_SIMT'] = '1'
-    try:
-        for m in model.conv_modules():
-            m._packed = None
-        ref = model(feats, coors, mask)
-    finally:
-        del os.environ['SE3B200_FORCE_SIMT']
+    ref, kinds = _forward_simt(model, feats, coors, mask)
+    assert 'pairwise_simt' in kinds and not kinds & {'pairwise_tc', 'pairwise_lr', 'zgemm'}, kinds
     for d in ('0', '1'):
         err = rel_err(out[d].cpu().numpy(), ref[d].cpu().numpy())
         assert err < TOL, f'degree {d}: {err:.3e}'
     # the production path captures in a CUDA graph (no host synchronisation inside the forward; the plan's run-time check is a
     # device-side flag read after the replay): replay == eager, bit for bit, also for new inputs of the same shape
-    for m in model.conv_modules():
-        m._packed = None
     eager = model(feats, coors, mask)
     graphed = model.graphed(feats, coors, mask)
     rep = graphed(feats, coors, mask)
@@ -175,7 +180,7 @@ def test_plan_guard_bounds_the_output_error(radial, monkeypatch):
     below the guard -- must match the direct K = 128 kernels of an identical model within 1e-4, and the first rejected one must
     raise LowRankPlanMiss instead of returning a degraded result.  The (residual, output error) pairs are recorded."""
     import json
-    from se3_transformer_pytorch_b200 import SE3Transformer, ops, model as M
+    from se3_transformer_pytorch_b200 import SE3Transformer, ops, switches, model as M
     if not ops.tc_supported(DEV, 128, 1):
         pytest.skip('needs sm_90')
     if radial == 'mlp':
@@ -187,11 +192,8 @@ def test_plan_guard_bounds_the_output_error(radial, monkeypatch):
     torch.manual_seed(5)
     with torch.device(DEV):
         planned = SE3Transformer(**ctor).eval()
-    os.environ['SE3B200_LOWRANK_MIN_EDGES'] = '0'
-    try:
+    with switches.override(lowrank_min_edges=0):
         planned.pack_weights(free_master=True, max_distance=2.0)
-    finally:
-        del os.environ['SE3B200_LOWRANK_MIN_EDGES']
     g = torch.Generator().manual_seed(9)
     n = 96
     feats = torch.randn(1, n, 128, generator=g).to(DEV)
@@ -200,11 +202,8 @@ def test_plan_guard_bounds_the_output_error(radial, monkeypatch):
     rows, accepted, rejected = [], 0, 0
     for scale in (1.0, 2.0, 3.0, 4.0, 4.2, 4.4, 4.5, 4.6, 4.7, 4.8, 4.9, 5.0, 6.0, 10.0, 40.0):
         coors = base * scale
-        os.environ['SE3B200_NO_LOWRANK'] = '1'
-        try:
+        with switches.override(no_lowrank=True):
             ref = direct(feats, coors, mask)
-        finally:
-            del os.environ['SE3B200_NO_LOWRANK']
         try:
             out = planned(feats, coors, mask)
         except M.LowRankPlanMiss:

@@ -21,8 +21,9 @@ def test_state_dict_layout_matches_reference(name):
     assert mine == state_keys(name)
 
 
-def test_library_exports_every_declared_symbol():
-    """The C-ABI library loads on a GPU-less box and exports everything include/se3b200.h declares."""
+def test_library_matches_header_at_abi_version_2():
+    """The C-ABI library loads on a GPU-less box, exports everything include/se3b200.h declares and reports ABI version 2
+    (se3_linear_tc_fwd takes flush_stages; the strided low-rank entry point is gone)."""
     from se3_transformer_pytorch_b200 import build, ops
     path = build.build()
     handle = ctypes.CDLL(path)
@@ -32,7 +33,7 @@ def test_library_exports_every_declared_symbol():
     for sym in declared:
         assert hasattr(handle, sym), f'{sym} declared in se3b200.h but not exported'
     assert declared == set(ops.EXPORTED_SYMBOLS)
-    assert ops.lib().se3_abi_version() == 1
+    assert ops.lib().se3_abi_version() == 2
 
 
 def test_build_stamp_survives_a_move_of_the_tree(tmp_path):
