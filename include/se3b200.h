@@ -51,7 +51,9 @@ int         se3_abi_version(void);     /* 2; raised with every incompatible chan
  *   modified = true distance; user neighbor_mask==0 -> FLT_MAX (S:1257); bonded (sparse_adj!=0) -> 0 (S:1262);
  *   causal and j' >= i on the self-removed grid -> FLT_MAX (S:1266-1268).
  * out_mask = (modified <= valid_radius) & node_mask[i] & node_mask[j]  (S:1284, 1290-1291).
- * node_mask, neighbor_mask, sparse_adj may be NULL.  Requires 1 <= k <= n-1 and n-1 <= 4096. */
+ * node_mask, neighbor_mask, sparse_adj may be NULL.  Requires 1 <= b <= 65535 and 1 <= k <= min(n-1, 4096); n is bounded by
+ * the grid only (one CTA per node).  A row of up to 4096 columns is sorted whole in shared memory; a longer row is searched in
+ * tiles of 4096 columns merged into a running list of the best next_pow2(k) keys, with the same keys, tie rule and results. */
 int se3_knn_fwd(const float* coors, const uint8_t* node_mask, const uint8_t* neighbor_mask, const uint8_t* sparse_adj,
                 int b, int n, int k, float valid_radius, int causal,
                 int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream);

@@ -1,8 +1,9 @@
 // K1: neighbour graph, pair-feature gather and masked-mean pooling.
 //
 // Replaces the dense [b,n,n-1] temporaries + torch.topk + batched_index_select of the reference
-// (se3_transformer_pytorch.py:1171-1294, utils.py:56-80) with one CTA per query node that keeps the whole
-// distance row in shared memory, sorts (distance, column) keys bitonically and emits only the k winners.  The same row body
+// (se3_transformer_pytorch.py:1171-1294, utils.py:56-80) with one CTA per query node that sorts (distance, column) keys of its
+// row bitonically in shared memory and emits only the k winners.  A row of up to KNN_TILE columns is sorted whole; a longer one
+// is walked in tiles of KNN_TILE columns, each merged into a running list of the best next_pow2(k) keys.  The same row body
 // serves padded batches [b, n] (knn_kernel) and packed batches of clouds of different sizes (knn_varlen_kernel).
 #include "common.cuh"
 #include <cfloat>
@@ -10,27 +11,31 @@
 
 namespace se3 {
 
+constexpr int KNN_TILE = 4096;      // columns per shared-memory sort; also the largest k (the running list sits next to the tile)
+
+__host__ __device__ inline int next_pow2(int v) {
+  int p = 1;
+  while (p < v) p <<= 1;
+  return p;
+}
+
 __host__ __device__ inline int knn_npad(int n) {
   int npad = 2;
   while (npad < n - 1) npad <<= 1;
   return npad;
 }
 
-// The neighbour list of node i of one cloud of n nodes (c = that cloud's coordinates, [n, 3]); shared by the padded
-// (knn_kernel) and the packed (knn_varlen_kernel) search so that both produce the same bits.
-// key = (bits(modified distance) << 32) | column on the self-removed grid.  Distances are >= 0 so the IEEE bit pattern is
-// order preserving; equal distances order by column, which is the stable-argsort tie rule the oracle uses (torch.topk
-// leaves ties unspecified).  nbr_row / adj_row: row i of the cloud's [n, n] pair masks (or NULL); node_mask: the cloud's
-// [n] node mask (or NULL).  Writes slots [0, K_out) of the row at out_*; slots r >= k are copies of slot k - 1 with mask 0,
-// and indices are offset by j_base.
+// keys[0, width) <- the keys of the self-removed columns [t0, t0 + width) of row i, ~0 past the last column.
+// key = (bits(modified distance) << 32) | column.  Distances are >= 0 so the IEEE bit pattern is order preserving; equal
+// distances order by column, which is the stable-argsort tie rule the oracle uses (torch.topk leaves ties unspecified).
+// Returns whether this thread wrote a key below `kth`.
 template <int THREADS>
-__device__ __forceinline__ void knn_row(unsigned long long* keys, const float* __restrict__ c, int n, int i, int k, int npad,
-                                        const uint8_t* __restrict__ nbr_row, const uint8_t* __restrict__ adj_row,
-                                        const uint8_t* __restrict__ node_mask, float valid_radius, int causal, int K_out,
-                                        int64_t j_base, int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
-                                        float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
-  const float xi = c[i * 3 + 0], yi = c[i * 3 + 1], zi = c[i * 3 + 2];
-  for (int jc = threadIdx.x; jc < npad; jc += THREADS) {
+__device__ __forceinline__ bool knn_tile_keys(unsigned long long* keys, const float* __restrict__ c, int n, int i, float xi,
+                                              float yi, float zi, int t0, int width, const uint8_t* __restrict__ nbr_row,
+                                              const uint8_t* __restrict__ adj_row, int causal, unsigned long long kth) {
+  bool below = false;
+  for (int t = threadIdx.x; t < width; t += THREADS) {
+    const int jc = t0 + t;
     unsigned long long key = ~0ull;
     if (jc < n - 1) {
       const int j = jc + (jc >= i);
@@ -41,10 +46,15 @@ __device__ __forceinline__ void knn_row(unsigned long long* keys, const float* _
       if (causal && jc >= i) d = FLT_MAX;
       key = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)jc;
     }
-    keys[jc] = key;
+    keys[t] = key;
+    below |= key < kth;
   }
-  __syncthreads();
-  // bitonic sort, ascending
+  return below;
+}
+
+// bitonic sort of keys[0, npad), ascending; npad a power of two
+template <int THREADS>
+__device__ __forceinline__ void knn_sort(unsigned long long* keys, int npad) {
   for (int size = 2; size <= npad; size <<= 1) {
     for (int stride = size >> 1; stride > 0; stride >>= 1) {
       for (int t = threadIdx.x; t < (npad >> 1); t += THREADS) {
@@ -57,9 +67,54 @@ __device__ __forceinline__ void knn_row(unsigned long long* keys, const float* _
       __syncthreads();
     }
   }
+}
+
+// The neighbour list of node i of one cloud of n nodes (c = that cloud's coordinates, [n, 3]); shared by the padded
+// (knn_kernel) and the packed (knn_varlen_kernel) search so that both produce the same bits.  nbr_row / adj_row: row i of the
+// cloud's [n, n] pair masks (or NULL); node_mask: the cloud's [n] node mask (or NULL).  Writes slots [0, K_out) of the row at
+// out_*; slots r >= k are copies of slot k - 1 with mask 0, and indices are offset by j_base.
+// keys: npad = next_pow2(n - 1) keys of shared memory when n - 1 <= KNN_TILE (one sort of the whole row), otherwise
+// KNN_TILE + next_pow2(k) keys (tile, then running list).  Keys are unique, so every top-k order gives the bits of one full sort.
+template <int THREADS>
+__device__ __forceinline__ void knn_row(unsigned long long* keys, const float* __restrict__ c, int n, int i, int k, int npad,
+                                        const uint8_t* __restrict__ nbr_row, const uint8_t* __restrict__ adj_row,
+                                        const uint8_t* __restrict__ node_mask, float valid_radius, int causal, int K_out,
+                                        int64_t j_base, int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
+                                        float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
+  const float xi = c[i * 3 + 0], yi = c[i * 3 + 1], zi = c[i * 3 + 2];
+  const unsigned long long* best = keys;
+  if (n - 1 <= KNN_TILE) {
+    knn_tile_keys<THREADS>(keys, c, n, i, xi, yi, zi, 0, npad, nbr_row, adj_row, causal, 0ull);
+    __syncthreads();
+    knn_sort<THREADS>(keys, npad);
+  } else {
+    unsigned long long* list = keys + KNN_TILE;      // the kpad smallest keys of the tiles so far, ascending
+    const int kpad = next_pow2(k);
+    for (int t = threadIdx.x; t < kpad; t += THREADS) list[t] = ~0ull;
+    for (int t0 = 0; t0 < n - 1; t0 += KNN_TILE) {
+      const unsigned long long kth = t0 ? list[k - 1] : ~0ull;
+      const bool below = knn_tile_keys<THREADS>(keys, c, n, i, xi, yi, zi, t0, KNN_TILE, nbr_row, adj_row, causal, kth);
+      if (__syncthreads_count(below) == 0) continue;   // nothing in this tile beats the current k-th key
+      knn_sort<THREADS>(keys, KNN_TILE);
+      // bitonic merge: min of the ascending list and the tile's first kpad keys reversed is a bitonic sequence of the kpad
+      // smallest keys of both; log2(kpad) half-cleaner stages sort it
+      for (int t = threadIdx.x; t < kpad; t += THREADS) list[t] = min(list[t], keys[kpad - 1 - t]);
+      __syncthreads();
+      for (int stride = kpad >> 1; stride > 0; stride >>= 1) {
+        for (int t = threadIdx.x; t < (kpad >> 1); t += THREADS) {
+          const int lo = 2 * t - (t & (stride - 1));
+          const int hi = lo + stride;
+          const unsigned long long a = list[lo], bb = list[hi];
+          if (a > bb) { list[lo] = bb; list[hi] = a; }
+        }
+        __syncthreads();
+      }
+    }
+    best = list;
+  }
   const bool mi = node_mask ? node_mask[i] != 0 : true;
   for (int r = threadIdx.x; r < K_out; r += THREADS) {
-    const unsigned long long key = keys[r < k ? r : k - 1];
+    const unsigned long long key = best[r < k ? r : k - 1];
     const int jc = (int)(key & 0xffffffffu);
     const float dmod = __uint_as_float((unsigned)(key >> 32));
     const int j = jc + (jc >= i);
@@ -76,9 +131,10 @@ __device__ __forceinline__ void knn_row(unsigned long long* keys, const float* _
   }
 }
 
-// One CTA per (cloud, node i) of a padded batch [b, n].
+// One CTA per (cloud, node i) of a padded batch [b, n].  Both kernels ask for 6 CTAs per SM: without it the tiled branch of
+// knn_row raises them from 40 to 48 registers, and whole-row searches would lose a CTA per SM.
 template <int THREADS>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 6)
 knn_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mask,
            const uint8_t* __restrict__ neighbor_mask, const uint8_t* __restrict__ sparse_adj,
            int n, int k, int npad, float valid_radius, int causal,
@@ -97,7 +153,7 @@ knn_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mas
 // its cloud by binary search, searches that cloud only (local columns, the cloud's own k_c) and writes K >= k_c slots with
 // global indices.  Pair masks are the clouds' [n_c, n_c] matrices flattened end to end, cloud c starting at pair_off[c].
 template <int THREADS>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, 6)
 knn_varlen_kernel(const float* __restrict__ coors, const int64_t* __restrict__ cu_seqlens, const int* __restrict__ k_per_cloud,
                   const uint8_t* __restrict__ neighbor_mask, const uint8_t* __restrict__ sparse_adj,
                   const int64_t* __restrict__ pair_off, int num_clouds, int K, float valid_radius, int causal,
@@ -157,11 +213,16 @@ extern "C" int se3_knn_fwd(const float* coors, const uint8_t* node_mask, const u
   using namespace se3;
   SE3_REQUIRE(b > 0 && n > 1, "se3_knn_fwd: need b > 0 and n > 1 (got b=%d n=%d)", b, n);
   SE3_REQUIRE(k >= 1 && k <= n - 1, "se3_knn_fwd: k must be in [1, n-1] (got k=%d n=%d)", k, n);
-  SE3_REQUIRE(n - 1 <= 4096, "se3_knn_fwd: n-1 = %d exceeds the 4096-column shared-memory sort", n - 1);
-  const int npad = knn_npad(n);
+  SE3_REQUIRE(b <= 65535, "se3_knn_fwd: b = %d exceeds the grid's y dimension (65535)", b);
+  SE3_REQUIRE(k <= KNN_TILE, "se3_knn_fwd: k = %d neighbours exceeds %d, the longest list the tiled search keeps in shared memory",
+              k, KNN_TILE);
   constexpr int THREADS = 256;
+  const bool tiled = n - 1 > KNN_TILE;
+  const int npad = tiled ? KNN_TILE : knn_npad(n);
+  const size_t smem = (size_t)(npad + (tiled ? next_pow2(k) : 0)) * sizeof(unsigned long long);
+  if (smem > 48 * 1024)
+    SE3_CUDA_OK(cudaFuncSetAttribute(knn_kernel<THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   dim3 grid(n, b);
-  const size_t smem = (size_t)npad * sizeof(unsigned long long);
   knn_kernel<THREADS><<<grid, THREADS, smem, as_stream(stream)>>>(coors, node_mask, neighbor_mask, sparse_adj, n, k, npad,
                                                                   valid_radius, causal, out_idx, out_mask, out_rel_pos,
                                                                   out_rel_dist);
