@@ -16,17 +16,20 @@
 //
 // MODE 3 evaluates the |m| > 0 case with three real products per complex one (Gauss): with c = x'[+m], d = x'[-m],
 //     S1 = sum (a+b) c,   S2 = sum a (d-c),   S3 = sum b (c+d);    out'[+] = S1 - S3,   out'[-] = S1 + S2
-// i.e. three accumulators, each fed by its own weight set (a+b, a, b) and its own Z: 3 instead of 4 K = 16 GEMM units per
-// (edge, o, i).  Chunk c of stage s belongs to weight set (4 s + c) % 3; the drain combines them.
+// i.e. three weight sets (a+b, a, b), each with its own Z: 3 instead of 4 K = 16 GEMM units per (edge, o, i).  The weight
+// image orders them set-major in blocks (zgauss_block): a segment's input channels in blocks of 4L, each block L stages of set
+// a+b, then L of set a, then L of set b.  One accumulator runs through a set; S1 of the block is kept in registers and
+// combined at the ends of sets a and b: -m += S1 + S2, +m += S1 - S3.
 //
-// CTA = 128 edges x NC channels (a slice of an N-wide tile of the weight image; MODE 1 / 4: NC = 128, one accumulator;
-// MODE 2: NC = 64, components (+m, -m) in two accumulators fed by the same B tiles; MODE 3: NC = 64, three accumulators).
+// CTA = 128 edges x NC channels (a slice of an N-wide tile of the weight image; MODE 1 / 3 / 4: NC = 128, one accumulator;
+// MODE 2: NC = 64, components (+m, -m) in two accumulators fed by the same B tiles).
 // 384 threads: warp 0 streams the weight image (TMA bulk copies into an mbarrier ring); warpgroups 1 and 2 own 64 edge rows
 // each, generate Z for their rows, issue m64 x NC x 16 wgmma with A from registers and B from shared memory, and keep the
-// fp32 partial sums: tensor-core accumulation truncates, so every `flush_stages` stages the accumulators are added into
-// registers with round-to-nearest adds and restarted.  MODE 1 / 3 commit one wgmma group per K chunk and generate the next chunk
-// while the previous chunks' MMAs are in flight, with X loaded into registers a stage (MODE 1) or a 3-stage period (MODE 3)
-// ahead; MODE 2 / 4 wait for their MMAs every stage.
+// fp32 partial sums: tensor-core accumulation truncates, so every `flush_stages` stages (MODE 3: also at the end of every set)
+// the accumulator is added into the partial sums with round-to-nearest adds and restarted.  MODE 3 keeps both of its planes
+// in shared memory (per-thread float4 slots) and S1 in registers.  MODE 1 / 3 commit one wgmma group per K chunk and
+// generate the next chunk while the previous chunks' MMAs are in flight, with X loaded into registers a stage ahead; MODE 2 / 4
+// wait for their MMAs every stage.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include <algorithm>
@@ -38,6 +41,26 @@ namespace se3 {
 constexpr int kZThreads = 384;
 constexpr int kZMaxSeg = 16;
 constexpr uint32_t kZWRingBytes = 196608;     // shared memory for the weight ring
+constexpr uint32_t kZSmemMax = 232448;        // dynamic shared memory of one CTA on sm_90
+
+// Shared memory of one CTA: 1 KiB alignment slack, the weight ring of WS stages, MODE 3's two planes (+m, -m) of fp32 partial
+// sums (64 floats per consumer thread each), the ring's mbarriers.  MODE 3 fills what is left after the planes with ring stages.
+template <int MODE, int NC>
+struct ZSmem {
+  static constexpr uint32_t kStageBytes = 2u * NC * 128u;                 // hi and lo rows of one stage
+  static constexpr uint32_t kPlaneBytes = (MODE == 3) ? 2u * 256u * 64u * 4u : 0u;
+  static constexpr uint32_t kRingBytes = (MODE == 3) ? kZSmemMax - 1024u - 256u - kPlaneBytes : kZWRingBytes;
+  static constexpr int WS = (kRingBytes / kStageBytes > 8) ? 8 : (int)(kRingBytes / kStageBytes);
+  static constexpr size_t kBytes = 1024 + (size_t)WS * kStageBytes + kPlaneBytes + 256;
+  static_assert(kBytes <= kZSmemMax, "shared memory");
+};
+
+// MODE 3 weight image: a segment's C_in input channels in blocks of 4L channels = 3L stages (L stages each of the weight sets
+// a+b, a, b; chunk c of stage w of a set = channel 4 w + c of the block).  L = the largest of 8, 4, 2, 1 that divides the
+// number of 4-channel groups, so that a set's accumulator takes at most 8 stages (96 K = 16 MMAs) before its drain.
+__host__ __device__ __forceinline__ int zgauss_block(int quads) {
+  return (quads % 8 == 0) ? 8 : (quads % 4 == 0) ? 4 : (quads % 2 == 0) ? 2 : 1;
+}
 
 template <int V>
 using ic = std::integral_constant<int, V>;
@@ -70,6 +93,16 @@ struct ZParams {
   int n_mt, n_nt, S, flush_stages;
 };
 
+// MODE 3's planes of fp32 partial sums: 16-byte slots in shared memory, kept in program order (one slot live at a time)
+__device__ __forceinline__ float4 lds128(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts128(uint32_t a, float4 v) {
+  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
+}
+
 // A fragment of one K = 16 chunk for rows (r0, r0 + 8), columns (kq, kq+1, kq+8, kq+9): v[row][4] -> fp16 hi / lo pairs
 __device__ __forceinline__ void z_frag(const float (&v)[2][4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
   split_h2(v[0][0], v[0][1], hi[0], lo[0]);
@@ -95,21 +128,24 @@ __device__ __forceinline__ void z_mma3(float (&d)[NR], const uint32_t (&hi)[4], 
 template <int MODE, int N, int NC>
 __global__ void __launch_bounds__(kZThreads, 1)
 zgemm_kernel(const __grid_constant__ ZParams prm) {
-  static_assert((MODE == 1 || MODE == 4) ? NC == 128 : NC == 64, "CTA width");
+  static_assert((MODE == 2) ? NC == 64 : NC == 128, "CTA width");
   static_assert(N % NC == 0 && (MODE == 1 || N == 128), "weight image tile");
-  constexpr int NA = (MODE == 3) ? 3 : (MODE == 2) ? 2 : 1;   // accumulators
+  constexpr int NA = (MODE == 2) ? 2 : 1;                      // accumulators
   constexpr int NO = (MODE == 2 || MODE == 3) ? 2 : 1;        // output planes
+  constexpr int NOR = (MODE == 3) ? 1 : NO;                    // fp32 planes in registers (MODE 3: S1; +m, -m in shared memory)
   constexpr int NR = NC / 2;                                   // fragment registers of one m64 x NC fp32 accumulator
   constexpr int NH = N / NC;                                   // CTAs per tile of the weight image
   constexpr uint32_t kImgStage = 2u * N * 128u;                // one stage of the weight image: [hi N rows | lo N rows] x 128 B
-  constexpr uint32_t kStageBytes = 2u * NC * 128u;             // what one CTA keeps of it: its NC rows of hi and of lo
-  constexpr int WS = (kZWRingBytes / kStageBytes > 8) ? 8 : (int)(kZWRingBytes / kStageBytes);
+  using SM = ZSmem<MODE, NC>;
+  constexpr uint32_t kStageBytes = SM::kStageBytes;            // what one CTA keeps of it: its NC rows of hi and of lo
+  constexpr int WS = SM::WS;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   const uint32_t sW = base;
-  const uint32_t bar_w_full = sW + WS * kStageBytes;
+  const uint32_t sPlane = sW + WS * kStageBytes;
+  const uint32_t bar_w_full = sPlane + SM::kPlaneBytes;
   const uint32_t bar_w_empty = bar_w_full + 8 * WS;
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
@@ -128,8 +164,11 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
   }
   __syncthreads();
 
+  // register split between the producer warpgroup and the two consumer warpgroups (128 x 40 + 256 x 232 or 128 x 24 + 256 x 240
+  // of the 64 K registers): MODE 3 holds the X of both components of a stage in flight and needs the larger consumer share
+  constexpr int kProdRegs = (MODE == 3) ? 24 : 40;
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProdRegs));
     if (warp == 0 && lane == 0) {
       // ===================== weight producer =====================
       const uint8_t* wsrc = prm.w_img + (size_t)nt * S * kImgStage + (size_t)hs * NC * 128u;
@@ -143,7 +182,7 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
     }
     return;
   }
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kProdRegs == 24 ? 240 : 232));
   // ===================== Z generators + MMA + fp32 partial sums =====================
   const int ct = threadIdx.x - 128;
   const int r0 = (ct >> 7) * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);    // rows r0, r0 + 8 of the edge tile
@@ -157,19 +196,24 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
     live[rs] = eg[rs] < prm.E;
     sxe[rs] = (live[rs] && MODE != 4) ? prm.sx[eg[rs]] : 1.f;
   }
-  float D[NA][NR], acc[NO][NR];
+  float D[NA][NR], acc[NOR][NR];
 #pragma unroll
   for (int a = 0; a < NA; ++a)
 #pragma unroll
     for (int j = 0; j < NR; ++j) D[a][j] = 0.f;
 #pragma unroll
-  for (int a = 0; a < NO; ++a)
+  for (int a = 0; a < NOR; ++a)
 #pragma unroll
     for (int j = 0; j < NR; ++j) acc[a][j] = 0.f;
+  // MODE 3's planes (+m at plane, -m at plane + 64 KiB): float4 slot g (fragment registers 4g .. 4g+3) of this thread at
+  // (g * 256 + ct) * 16 B, conflict-free
+  const uint32_t plane = sPlane + 16u * ct;
+  if constexpr (MODE == 3)
+#pragma unroll
+    for (int g = 0; g < NR / 2; ++g) sts128(plane + 4096u * g, make_float4(0.f, 0.f, 0.f, 0.f));
   int blk_start = 0;
   // MODE 1 / 3 restart a drained accumulator with the first MMA that writes it (scale-d = 0) instead of zeroing its registers,
-  // so D is written only by wgmma (bit a: accumulator a is drained).  Every stage writes every accumulator, so each block of
-  // flush_stages stages restarts all of them before the next drain.
+  // so D is written only by wgmma (bit a: accumulator a is drained).
   int fresh = 0;
 
   auto release = [&](int s) {                  // every MMA that read the weight slot of stage s has retired
@@ -181,13 +225,8 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
   auto drain = [&](int s) {
 #pragma unroll
     for (int j = 0; j < NR; ++j) {
-      if (MODE == 3) {
-        acc[0][j] += D[0][j] - D[NA - 1][j];
-        acc[1][j] += D[0][j] + D[NA > 1 ? 1 : 0][j];
-      } else {
 #pragma unroll
-        for (int a = 0; a < NA; ++a) acc[a][j] += D[a][j];
-      }
+      for (int a = 0; a < NA; ++a) acc[a][j] += D[a][j];
       if (MODE == 2 || MODE == 4)
 #pragma unroll
         for (int a = 0; a < NA; ++a) D[a][j] = 0.f;
@@ -205,7 +244,7 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
 
   // MODE 1 / 3: one commit group per K chunk, so the MMAs of the last ZR - 1 chunks stay in flight while the next chunk's A
   // fragments are generated
-  constexpr int ZR = (MODE == 3) ? 2 : 4;
+  constexpr int ZR = 4;
   float u[2][4];                               // U[e, kq, kq+1, kq+8, kq+9] * sx[e] of rows r0, r0 + 8 (current segment)
   auto zf = [&](const float (&y)[2], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
     float v[2][4];
@@ -371,47 +410,81 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
           finish_stage(s);
         }
       } else {
-        // K chunk q = 4 sl + c of the segment: input channel q / 3, weight set q % 3 of (a+b, a, b) <-> y = (c, d - c, c + d).  The
-        // map repeats every 3 stages (12 chunks, 4 input channels) and ns = 3 C_in / 4, so the loop runs over whole periods with
-        // every channel offset and accumulator index known at compile time.  Each (channel, +-m component, row) value is loaded
-        // once per period, one period ahead: channel j of the next period as soon as the last chunk of channel j is generated.
+        // set-major blocks (zgauss_block): stage w of set T of a block feeds input channels 4 w + c of the block to weight set T of
+        // (a+b, a, b) with y = (c, d - c, c + d), c = x'(+m), d = x'(-m).  As in MODE 1 the rows of chunk c are loaded one stage
+        // ahead; the next stage's channels are the next 4 of the set, the set's first 4 again (next set of the block) or the next
+        // block's first 4.
+        const int L = zgauss_block(z.Ci / 4);
         const int dmo = (z.cminus - z.cplus) * 128;                   // from x'(+m) to x'(-m) of the same channel
-        float x[4][2][2];                      // [channel of the period][c = x'(+m), d = x'(-m)][row]
+        const int step = 4 * z.ncomp * 128, rewind = -(L - 1) * step; // to the next 4 channels, back to the set's first 4
+        float x[4][2][2];                      // [chunk][c = x'(+m), d = x'(-m)][row]
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
+        for (int c = 0; c < 4; ++c)
 #pragma unroll
           for (int rs = 0; rs < 2; ++rs) {
-            x[j][0][rs] = __ldg(xp + j * istride + 8 * rs);
-            x[j][1][rs] = __ldg(xp + dmo + j * istride + 8 * rs);
+            x[c][0][rs] = __ldg(xp + c * istride + 8 * rs);
+            x[c][1][rs] = __ldg(xp + dmo + c * istride + 8 * rs);
           }
-        const int np = ns / 3;
+        int left = L - 1, set = 0;             // stages left in the set after this one, set of the block
+        bool set_open = false;                 // the current set has been drained before (S1 holds part of set a+b)
+        const int s_end = s + ns;
 #pragma unroll 1
-        for (int p = 0; p < np; ++p) {
-          const size_t adv = (p + 1 < np) ? 4 * istride : 0;          // the last period reloads its own rows, never past the tile
-          static_for<3>([&](auto tc) {
-            uint64_t b_hi, b_lo;
-            wait_stage(s, b_hi, b_lo);
-            static_for<4>([&](auto cc) {
-              constexpr int Q = 4 * decltype(tc)::value + decltype(cc)::value, J = Q / 3, T = Q % 3;
-              float y[2];
+        for (; s < s_end; ++s) {
+          const bool set_end = left == 0;
+          // the last stage reloads its own rows, never past the tile
+          const float* xn = (s + 1 == s_end) ? xp : xp + ((!set_end || set == 2) ? step : rewind);
+          const float fc = (set == 1) ? -1.f : 1.f, fd = (set == 0) ? 0.f : 1.f;     // y = fc c + fd d, rounded once
+          uint64_t b_hi, b_lo;
+          wait_stage(s, b_hi, b_lo);
+          static_for<4>([&](auto cc) {
+            constexpr int C = decltype(cc)::value;
+            float y[2];
 #pragma unroll
-              for (int rs = 0; rs < 2; ++rs) {
-                const float cp = x[J][0][rs], dm = x[J][1][rs];
-                y[rs] = (T == 0) ? cp : (T == 1) ? (dm - cp) : (cp + dm);
-              }
-              chunk_mma(cc, ic<T>(), s, y, b_hi, b_lo);
-              if constexpr (T == 2) {
+            for (int rs = 0; rs < 2; ++rs) y[rs] = fmaf(fc, x[C][0][rs], fd * x[C][1][rs]);
+            chunk_mma(cc, ic<0>(), s, y, b_hi, b_lo);
 #pragma unroll
-                for (int rs = 0; rs < 2; ++rs) {
-                  x[J][0][rs] = __ldg(xp + adv + J * istride + 8 * rs);
-                  x[J][1][rs] = __ldg(xp + adv + dmo + J * istride + 8 * rs);
-                }
-              }
-            });
-            end_stage(s);
-            ++s;
+            for (int rs = 0; rs < 2; ++rs) {
+              x[C][0][rs] = __ldg(xn + C * istride + 8 * rs);
+              x[C][1][rs] = __ldg(xn + dmo + C * istride + 8 * rs);
+            }
           });
-          xp += adv;
+          if (set_end || s + 1 - blk_start == FS) {
+            // S1 (set a+b) collects in registers; set a ends with -m += S1 + S2, set b with +m += S1 - S3 (a drain inside a set
+            // adds +-D alone)
+            wgmma_wait0();
+            release(s);
+            if (set == 0) {
+#pragma unroll
+              for (int j = 0; j < NR; ++j) acc[0][j] = set_open ? acc[0][j] + D[0][j] : D[0][j];
+            } else {
+              const uint32_t pl = plane + (set == 1 ? 65536u : 0u);
+#pragma unroll
+              for (int g = 0; g < NR / 4; ++g) {
+                float4 v = lds128(pl + 4096u * g);
+                float t[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                  const float d = D[0][4 * g + q], s1 = acc[0][4 * g + q];
+                  t[q] = set_end ? (set == 1 ? s1 + d : s1 - d) : (set == 1 ? d : -d);
+                }
+                v.x += t[0];
+                v.y += t[1];
+                v.z += t[2];
+                v.w += t[3];
+                sts128(pl + 4096u * g, v);
+              }
+            }
+            set_open = !set_end;
+            fresh = 1;
+            blk_start = s + 1;
+          }
+          xp = xn;
+          if (set_end) {
+            left = L - 1;
+            set = (set == 2) ? 0 : set + 1;
+          } else {
+            --left;
+          }
         }
       }
     }
@@ -425,8 +498,16 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
       for (int a = 0; a < NO; ++a) {
         float* dst = prm.out + (size_t)eg[rs] * prm.out_es + prm.comp_off[a] + (size_t)nt * N + (size_t)hs * NC + kq;
 #pragma unroll
-        for (int g = 0; g < NC / 8; ++g)
-          *reinterpret_cast<float2*>(dst + 8 * g) = make_float2(acc[a][4 * g + 2 * rs] * inv, acc[a][4 * g + 2 * rs + 1] * inv);
+        for (int g = 0; g < NC / 8; ++g) {
+          float2 v;
+          if (MODE == 3) {
+            const float4 q = lds128(plane + 65536u * a + 4096u * g);
+            v = rs ? make_float2(q.z, q.w) : make_float2(q.x, q.y);
+          } else {
+            v = make_float2(acc[a < NOR ? a : 0][4 * g + 2 * rs], acc[a < NOR ? a : 0][4 * g + 2 * rs + 1]);
+          }
+          *reinterpret_cast<float2*>(dst + 8 * g) = make_float2(v.x * inv, v.y * inv);
+        }
       }
     }
   }
@@ -434,19 +515,20 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
 
 // Weight image of one sub-segment: rows (o, i, f) of Fp (columns [col0, col0+16) of each row) -> stages [stage0, stage0+n) of
 // the launch image.  Chunk c = i*F + f of the segment sits in stage c/4 at K columns [(c%4)*16, +16).
-// gauss != 0 (MODE 3): Fp rows are (o, i, f in {a, b}); K chunk q = 4 sl + c of the segment = weight set q % 3 of (a+b, a, b) of
-// input channel q / 3.
+// gauss != 0 (MODE 3): Fp rows are (o, i, f in {a, b}); stage sl of the segment = stage w of weight set T of (a+b, a, b) of
+// block b (zgauss_block: sl = 3 L b + L T + w), its chunk c = input channel 4 L b + 4 w + c.
 __global__ void zpack_kernel(const float* __restrict__ Fp, int Kp, int col0, int Co, int CiF, int N, int S, int stage0, int n_stage,
                              int gauss, uint8_t* __restrict__ img) {
   const int nt = blockIdx.y, sl = blockIdx.x;
   uint8_t* dst = img + ((size_t)nt * S + stage0 + sl) * (2u * N * 128u);
+  const int L = gauss ? zgauss_block(n_stage / 3) : 1;
   for (int t = threadIdx.x; t < N * 64; t += blockDim.x) {
     const int r = t >> 6, k = t & 63;
     const int o = nt * N + r;
     float w = 0.f;
     if (gauss) {
-      const int q = sl * 4 + (k >> 4);
-      const int ty = q % 3, i = q / 3;
+      const int tb = sl % (3 * L);
+      const int ty = tb / L, i = (sl / (3 * L)) * 4 * L + 4 * (tb % L) + (k >> 4);
       if (2 * i + 1 < CiF && o < Co) {
         const float wa = Fp[((size_t)o * CiF + 2 * i) * Kp + col0 + (k & 15)], wb = Fp[((size_t)o * CiF + 2 * i + 1) * Kp + col0 + (k & 15)];
         w = (ty == 0) ? wa + wb : (ty == 1) ? wa : wb;
@@ -465,9 +547,7 @@ __global__ void zpack_kernel(const float* __restrict__ Fp, int Kp, int col0, int
 
 template <int MODE, int N, int NC>
 static int launch_z(const ZParams& prm, cudaStream_t s) {
-  constexpr uint32_t kStageBytes = 2u * NC * 128u;
-  constexpr int WS = (kZWRingBytes / kStageBytes > 8) ? 8 : (int)(kZWRingBytes / kStageBytes);
-  const size_t smem = 1024 + (size_t)WS * kStageBytes + 256;
+  const size_t smem = ZSmem<MODE, NC>::kBytes;
   auto kern = zgemm_kernel<MODE, N, NC>;
   SE3_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t grid = (int64_t)prm.n_mt * prm.n_nt * (N / NC);
@@ -579,11 +659,11 @@ extern "C" int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img,
   prm.n_mt = (int)ceil_div(E, SE3_TILE_E);
   prm.n_nt = Co / N;
   prm.S = S;
-  // default drain period: 96 accumulating K = 16 MMAs per accumulator (8 stages of 12; mode 3 spreads its stages over three
-  // accumulators): rel. error 4e-6 against float64 for all-positive operands at K = 65536 (2.5e-4 if never drained)
-  prm.flush_stages = flush_stages > 0 ? flush_stages : (mode == 3 ? 24 : 8);
+  // default drain period: 96 accumulating K = 16 MMAs per accumulator (8 stages of 12; mode 3 also drains at the end of every
+  // weight set, at most 8 stages): rel. error 4e-6 against float64 for all-positive operands at K = 65536 (2.5e-4 if never drained)
+  prm.flush_stages = flush_stages > 0 ? flush_stages : 8;
   cudaStream_t s = as_stream(stream);
-  if (mode == 3) return launch_z<3, 128, 64>(prm, s);
+  if (mode == 3) return launch_z<3, 128, 128>(prm, s);
   if (mode == 2) return launch_z<2, 128, 64>(prm, s);
   return N == 256 ? launch_z<1, 256, 128>(prm, s) : launch_z<1, 128, 128>(prm, s);
 }

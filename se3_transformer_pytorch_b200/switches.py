@@ -17,8 +17,8 @@ implementations of the same forward (or tunes one); none changes what the model 
 | SE3B200_NO_LINEAR_TC        | no_linear_tc      | off              | cuBLAS LinearSE3 instead of the tensor-core kernel                |
 | SE3B200_NO_ATTN_ROTATE      | no_attn_rotate    | off              | separate rotate-back instead of the one fused into attention      |
 | SE3B200_HOST_FRAMES         | host_frames       | off              | edge frames from the float64 torch code of aligned.py             |
-| SE3B200_Z_FLUSH             | z_flush           | unset            | tensor-core accumulator drain period in stages (unset: 24 for the |
-|                             |                   |                  | m > 0 GEMMs of mode 3, 8 for the others and for LinearSE3)        |
+| SE3B200_Z_FLUSH             | z_flush           | unset            | tensor-core accumulator drain period in stages (unset: 8; the     |
+|                             |                   |                  | m > 0 GEMMs of mode 3 also drain at the end of every weight set)  |
 | SE3B200_Z_FLUSH_MULT        | z_flush_mult      | 1                | multiplies the drain period of the ConvSE3 GEMMs                  |
 
 The model reads `current()` once per ConvSE3 dispatch, LinearSE3 / AttentionSE3 call, Geometry and pack_weights; ConvSE3
@@ -53,7 +53,7 @@ class Switches:
         """flush_stages of se3_zgemm_fwd: 0 (the library's default) unless SE3B200_Z_FLUSH or SE3B200_Z_FLUSH_MULT is set."""
         if self.z_flush is None and self.z_flush_mult == 1:
             return 0
-        base = self.z_flush if self.z_flush is not None else (24 if mode == 3 else 8)
+        base = self.z_flush if self.z_flush is not None else 8
         return max(1, base * max(1, self.z_flush_mult))
 
     def linear_flush(self):
