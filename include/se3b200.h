@@ -6,6 +6,7 @@
  *
  *   neighbour builder inside SE3Transformer.forward   se3_transformer_pytorch.py:1171-1294  -> se3_knn_fwd
  *     (packed batches of clouds of different sizes, SE3Transformer.forward_packed: se3_knn_varlen_fwd; no reference counterpart)
+ *     (sparse pair inputs: se3_knn_csr_fwd and se3_pair_lookup_fwd; no reference counterpart)
  *   get_basis(r_ij, max_degree)                        basis.py:153-205                      -> se3_basis_fwd
  *   RadialFunc trunk (net.0 .. net.5)                  se3_transformer_pytorch.py:287-293    -> se3_radial_trunk_fwd
  *   PairwiseConv + ConvSE3 inner product               se3_transformer_pytorch.py:237-254,
@@ -71,6 +72,24 @@ int se3_knn_varlen_fwd(const float* coors, const int64_t* cu_seqlens, const int*
                        const uint8_t* sparse_adj, const int64_t* pair_off, int num_clouds, int64_t total, int K, int max_len,
                        float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos,
                        float* out_rel_dist, void* stream);
+
+/* se3_knn_fwd with the pair masks given as sparse rows instead of [b, n, n] bytes (SE3Transformer.forward with torch.sparse_coo
+ * pair inputs).  A list is int64 row pointers ptr and int32 columns cols [nnz]: row (b, i) is cols[ptr[r] .. ptr[r+1]) with
+ * r = b * batch_stride + i, columns ascending and unique per row (a diagonal entry is allowed and ignored).  batch_stride is n
+ * (ptr has b*n + 1 entries) or 0 (ptr has n + 1 entries: one list shared by the batch).  A column listed in row (b, i) of the
+ * neighbour list is allowed and one missing from it gets distance FLT_MAX; a column of the bonded list gets distance 0; causal
+ * overrides both -- the precedence, keys, tie rule and results of se3_knn_fwd on the densified masks, bit for bit.  Either list
+ * may be NULL (cols == NULL); rows have no length limit.  Row pointers are clamped to [0, nnz]. */
+int se3_knn_csr_fwd(const float* coors, const uint8_t* node_mask, const int64_t* nbr_ptr, const int* nbr_cols, int64_t nbr_nnz,
+                    int64_t nbr_batch_stride, const int64_t* adj_ptr, const int* adj_cols, int64_t adj_nnz,
+                    int64_t adj_batch_stride, int b, int n, int k, float valid_radius, int causal, int64_t* out_idx,
+                    uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream);
+
+/* Position of every neighbour in a sparse pair list (row pointers and columns as in se3_knn_csr_fwd): out[b,i,kk] = p with
+ * cols[p] == idx[b,i,kk] inside row (b, i), or -1 if the row lacks that column.  idx, out: [b, n, k] int64.  The caller indexes
+ * the list's values (edge tokens, edge features, hop counts) with a zero row appended for -1. */
+int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx, int b, int n,
+                        int k, int64_t* out, void* stream);
 
 /* Gather per-pair features onto the neighbour list (batched_index_select at S:1293-1294, utils.py:56-70):
  * out[b,i,kk,:] = pair_feat[b,i,idx[b,i,kk],:]   with pair_feat [b,n,n,e]. */

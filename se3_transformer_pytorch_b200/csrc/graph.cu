@@ -4,7 +4,8 @@
 // (se3_transformer_pytorch.py:1171-1294, utils.py:56-80) with one CTA per query node that sorts (distance, column) keys of its
 // row bitonically in shared memory and emits only the k winners.  A row of up to KNN_TILE columns is sorted whole; a longer one
 // is walked in tiles of KNN_TILE columns, each merged into a running list of the best next_pow2(k) keys.  The same row body
-// serves padded batches [b, n] (knn_kernel) and packed batches of clouds of different sizes (knn_varlen_kernel).
+// serves padded batches [b, n] (knn_kernel), packed batches of clouds of different sizes (knn_varlen_kernel) and pair masks
+// given as sorted column lists (knn_csr_kernel; pair_lookup_kernel finds a neighbour's pair in such a list).
 #include "common.cuh"
 #include <cfloat>
 #include <vector>
@@ -25,14 +26,69 @@ __host__ __device__ inline int knn_npad(int n) {
   return npad;
 }
 
+// Where the pair row of node i comes from.  DensePairs: row i of the cloud's [n, n] byte masks (or NULL).  CsrPairs: the sorted
+// column lists of row i, staged tile by tile into shared-memory bitmaps.  Both answer, for a column j != i of the current tile,
+// whether j is outside the neighbour mask and whether it is bonded; knn_tile_keys applies the answers in the same order.
+struct DensePairs {
+  const uint8_t* __restrict__ nbr;
+  const uint8_t* __restrict__ adj;
+  template <int THREADS>
+  __device__ __forceinline__ void stage(int, int) {}
+  __device__ __forceinline__ bool excluded(int j) const { return nbr && !nbr[j]; }
+  __device__ __forceinline__ bool bonded(int j) const { return adj && adj[j]; }
+};
+
+constexpr int CSR_BITMAP_WORDS = KNN_TILE / 32 + 1;   // columns j in [t0, t0 + KNN_TILE] of one tile (self removed: one extra)
+
+// first position p in [lo, hi) with cols[p] >= v (hi if none)
+__device__ __forceinline__ int64_t csr_lower_bound(const int* __restrict__ cols, int64_t lo, int64_t hi, int v) {
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (cols[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+struct CsrPairs {
+  const int* __restrict__ nbr;       // columns of the neighbour mask (NULL: no mask); row entries [nbr_lo, nbr_hi)
+  const int* __restrict__ adj;       // columns of the bonded neighbours (NULL: none); row entries [adj_lo, adj_hi)
+  int64_t nbr_lo, nbr_hi, adj_lo, adj_hi;
+  unsigned* bits;                    // 2 x CSR_BITMAP_WORDS words of shared memory: neighbour mask, then bonded
+  int t0;
+
+  template <int THREADS>
+  __device__ __forceinline__ void scatter(const int* __restrict__ cols, int64_t lo, int64_t hi, unsigned* words, int width) {
+    // only the row's entries inside this tile are read; an entry outside [t0, t0 + width] never touches the bitmap
+    const int64_t first = csr_lower_bound(cols, lo, hi, t0);
+    for (int64_t p = first + threadIdx.x; p < hi; p += THREADS) {
+      const int c = cols[p];
+      if (c > t0 + width) break;
+      if (c >= t0) atomicOr(&words[(c - t0) >> 5], 1u << ((c - t0) & 31));
+    }
+  }
+  // bits <- the row's entries among the columns of tile [t0, t0 + width) (self-removed positions, so columns t0 .. t0 + width)
+  template <int THREADS>
+  __device__ __forceinline__ void stage(int tile0, int width) {
+    t0 = tile0;
+    for (int w = threadIdx.x; w < 2 * CSR_BITMAP_WORDS; w += THREADS) bits[w] = 0u;
+    __syncthreads();
+    if (nbr) scatter<THREADS>(nbr, nbr_lo, nbr_hi, bits, width);
+    if (adj) scatter<THREADS>(adj, adj_lo, adj_hi, bits + CSR_BITMAP_WORDS, width);
+    __syncthreads();
+  }
+  __device__ __forceinline__ bool bit(const unsigned* words, int j) const { return (words[(j - t0) >> 5] >> ((j - t0) & 31)) & 1u; }
+  __device__ __forceinline__ bool excluded(int j) const { return nbr && !bit(bits, j); }
+  __device__ __forceinline__ bool bonded(int j) const { return adj && bit(bits + CSR_BITMAP_WORDS, j); }
+};
+
 // keys[0, width) <- the keys of the self-removed columns [t0, t0 + width) of row i, ~0 past the last column.
 // key = (bits(modified distance) << 32) | column.  Distances are >= 0 so the IEEE bit pattern is order preserving; equal
 // distances order by column, which is the stable-argsort tie rule the oracle uses (torch.topk leaves ties unspecified).
 // Returns whether this thread wrote a key below `kth`.
-template <int THREADS>
+template <int THREADS, class Pairs>
 __device__ __forceinline__ bool knn_tile_keys(unsigned long long* keys, const float* __restrict__ c, int n, int i, float xi,
-                                              float yi, float zi, int t0, int width, const uint8_t* __restrict__ nbr_row,
-                                              const uint8_t* __restrict__ adj_row, int causal, unsigned long long kth) {
+                                              float yi, float zi, int t0, int width, const Pairs& pairs, int causal,
+                                              unsigned long long kth) {
   bool below = false;
   for (int t = threadIdx.x; t < width; t += THREADS) {
     const int jc = t0 + t;
@@ -41,8 +97,8 @@ __device__ __forceinline__ bool knn_tile_keys(unsigned long long* keys, const fl
       const int j = jc + (jc >= i);
       const float dx = xi - c[j * 3 + 0], dy = yi - c[j * 3 + 1], dz = zi - c[j * 3 + 2];
       float d = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
-      if (nbr_row && !nbr_row[j]) d = FLT_MAX;
-      if (adj_row && adj_row[j]) d = 0.f;
+      if (pairs.excluded(j)) d = FLT_MAX;
+      if (pairs.bonded(j)) d = 0.f;
       if (causal && jc >= i) d = FLT_MAX;
       key = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)jc;
     }
@@ -70,21 +126,21 @@ __device__ __forceinline__ void knn_sort(unsigned long long* keys, int npad) {
 }
 
 // The neighbour list of node i of one cloud of n nodes (c = that cloud's coordinates, [n, 3]); shared by the padded
-// (knn_kernel) and the packed (knn_varlen_kernel) search so that both produce the same bits.  nbr_row / adj_row: row i of the
-// cloud's [n, n] pair masks (or NULL); node_mask: the cloud's [n] node mask (or NULL).  Writes slots [0, K_out) of the row at
-// out_*; slots r >= k are copies of slot k - 1 with mask 0, and indices are offset by j_base.
+// (knn_kernel), the packed (knn_varlen_kernel) and the CSR (knn_csr_kernel) search so that all produce the same bits.  pairs:
+// row i of the cloud's pair masks (DensePairs or CsrPairs); node_mask: the cloud's [n] node mask (or NULL).  Writes slots
+// [0, K_out) of the row at out_*; slots r >= k are copies of slot k - 1 with mask 0, and indices are offset by j_base.
 // keys: npad = next_pow2(n - 1) keys of shared memory when n - 1 <= KNN_TILE (one sort of the whole row), otherwise
 // KNN_TILE + next_pow2(k) keys (tile, then running list).  Keys are unique, so every top-k order gives the bits of one full sort.
-template <int THREADS>
+template <int THREADS, class Pairs>
 __device__ __forceinline__ void knn_row(unsigned long long* keys, const float* __restrict__ c, int n, int i, int k, int npad,
-                                        const uint8_t* __restrict__ nbr_row, const uint8_t* __restrict__ adj_row,
-                                        const uint8_t* __restrict__ node_mask, float valid_radius, int causal, int K_out,
+                                        Pairs pairs, const uint8_t* __restrict__ node_mask, float valid_radius, int causal, int K_out,
                                         int64_t j_base, int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
                                         float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
   const float xi = c[i * 3 + 0], yi = c[i * 3 + 1], zi = c[i * 3 + 2];
   const unsigned long long* best = keys;
   if (n - 1 <= KNN_TILE) {
-    knn_tile_keys<THREADS>(keys, c, n, i, xi, yi, zi, 0, npad, nbr_row, adj_row, causal, 0ull);
+    pairs.template stage<THREADS>(0, npad);
+    knn_tile_keys<THREADS>(keys, c, n, i, xi, yi, zi, 0, npad, pairs, causal, 0ull);
     __syncthreads();
     knn_sort<THREADS>(keys, npad);
   } else {
@@ -93,7 +149,8 @@ __device__ __forceinline__ void knn_row(unsigned long long* keys, const float* _
     for (int t = threadIdx.x; t < kpad; t += THREADS) list[t] = ~0ull;
     for (int t0 = 0; t0 < n - 1; t0 += KNN_TILE) {
       const unsigned long long kth = t0 ? list[k - 1] : ~0ull;
-      const bool below = knn_tile_keys<THREADS>(keys, c, n, i, xi, yi, zi, t0, KNN_TILE, nbr_row, adj_row, causal, kth);
+      pairs.template stage<THREADS>(t0, KNN_TILE);
+      const bool below = knn_tile_keys<THREADS>(keys, c, n, i, xi, yi, zi, t0, KNN_TILE, pairs, causal, kth);
       if (__syncthreads_count(below) == 0) continue;   // nothing in this tile beats the current k-th key
       knn_sort<THREADS>(keys, KNN_TILE);
       // bitonic merge: min of the ascending list and the tile's first kpad keys reversed is a bitonic sequence of the kpad
@@ -144,9 +201,39 @@ knn_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mas
   const int i = blockIdx.x, b = blockIdx.y;
   const size_t row = ((size_t)b * n + i) * n;
   const size_t o = ((size_t)b * n + i) * k;
-  knn_row<THREADS>(keys, coors + (size_t)b * n * 3, n, i, k, npad, neighbor_mask ? neighbor_mask + row : nullptr,
-                   sparse_adj ? sparse_adj + row : nullptr, node_mask ? node_mask + (size_t)b * n : nullptr, valid_radius, causal,
-                   k, 0, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
+  knn_row<THREADS>(keys, coors + (size_t)b * n * 3, n, i, k, npad,
+                   DensePairs{neighbor_mask ? neighbor_mask + row : nullptr, sparse_adj ? sparse_adj + row : nullptr},
+                   node_mask ? node_mask + (size_t)b * n : nullptr, valid_radius, causal, k, 0, out_idx + o, out_mask + o,
+                   out_rel_pos + o * 3, out_rel_dist + o);
+}
+
+// knn_kernel with the pair masks given as CSR rows: row (b, i) of a list is entries [ptr[r], ptr[r+1]) of its columns, with
+// r = b * batch_stride + i (batch_stride 0: one [n, n] list shared by the batch).  Row pointers are clamped to [0, nnz], so a
+// malformed list reads no memory outside it.  Shared memory: the keys of knn_kernel, then the two bitmaps of CsrPairs.
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS, 6)
+knn_csr_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mask,
+               const int64_t* __restrict__ nbr_ptr, const int* __restrict__ nbr_cols, int64_t nbr_nnz, int64_t nbr_stride,
+               const int64_t* __restrict__ adj_ptr, const int* __restrict__ adj_cols, int64_t adj_nnz, int64_t adj_stride,
+               int n, int k, int npad, int key_words, float valid_radius, int causal,
+               int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
+               float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
+  extern __shared__ unsigned long long keys[];
+  const int i = blockIdx.x, b = blockIdx.y;
+  const size_t o = ((size_t)b * n + i) * k;
+  CsrPairs pairs{nbr_cols, adj_cols, 0, 0, 0, 0, reinterpret_cast<unsigned*>(keys + key_words), 0};
+  if (nbr_cols) {
+    const int64_t r = (int64_t)b * nbr_stride + i;
+    pairs.nbr_lo = min(max(nbr_ptr[r], (int64_t)0), nbr_nnz);
+    pairs.nbr_hi = min(max(nbr_ptr[r + 1], pairs.nbr_lo), nbr_nnz);
+  }
+  if (adj_cols) {
+    const int64_t r = (int64_t)b * adj_stride + i;
+    pairs.adj_lo = min(max(adj_ptr[r], (int64_t)0), adj_nnz);
+    pairs.adj_hi = min(max(adj_ptr[r + 1], pairs.adj_lo), adj_nnz);
+  }
+  knn_row<THREADS>(keys, coors + (size_t)b * n * 3, n, i, k, npad, pairs, node_mask ? node_mask + (size_t)b * n : nullptr,
+                   valid_radius, causal, k, 0, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
 }
 
 // One CTA per node of a packed batch: clouds c of n_c = cu_seqlens[c+1] - cu_seqlens[c] nodes laid end to end.  The CTA finds
@@ -170,9 +257,9 @@ knn_varlen_kernel(const float* __restrict__ coors, const int64_t* __restrict__ c
   const int n = (int)(cu_seqlens[lo + 1] - start), i = (int)(t - start);
   const size_t row = neighbor_mask || sparse_adj ? (size_t)pair_off[lo] + (size_t)i * n : 0;
   const size_t o = (size_t)t * K;
-  knn_row<THREADS>(keys, coors + start * 3, n, i, k_per_cloud[lo], knn_npad(n), neighbor_mask ? neighbor_mask + row : nullptr,
-                   sparse_adj ? sparse_adj + row : nullptr, nullptr, valid_radius, causal, K, start, out_idx + o, out_mask + o,
-                   out_rel_pos + o * 3, out_rel_dist + o);
+  knn_row<THREADS>(keys, coors + start * 3, n, i, k_per_cloud[lo], knn_npad(n),
+                   DensePairs{neighbor_mask ? neighbor_mask + row : nullptr, sparse_adj ? sparse_adj + row : nullptr}, nullptr,
+                   valid_radius, causal, K, start, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
 }
 
 __global__ void gather_pairs_kernel(const float* __restrict__ pf, const int64_t* __restrict__ idx, int n, int k, int e,
@@ -184,6 +271,23 @@ __global__ void gather_pairs_kernel(const float* __restrict__ pf, const int64_t*
   const int64_t bi = edge / k;              // b*n + i
   const int64_t j = idx[edge];
   out[t] = pf[(bi * n + j) * e + c];
+}
+
+// out[s] = position of column idx[s] in CSR row s / k (clamped to [0, nnz] as in knn_csr_kernel), or -1 if the row lacks it.
+__global__ void pair_lookup_kernel(const int64_t* __restrict__ ptr, const int* __restrict__ cols, int64_t nnz, int64_t stride,
+                                   const int64_t* __restrict__ idx, int n, int k, int64_t total, int64_t* __restrict__ out) {
+  const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= total) return;
+  const int64_t bi = s / k;                  // b * n + i
+  const int64_t r = (bi / n) * stride + bi % n;
+  const int64_t lo = min(max(ptr[r], (int64_t)0), nnz), hi = min(max(ptr[r + 1], lo), nnz);
+  const int64_t j = idx[s];
+  int64_t pos = -1;
+  if (j >= 0 && j < n) {
+    const int64_t p = csr_lower_bound(cols, lo, hi, (int)j);
+    if (p < hi && cols[p] == (int)j) pos = p;
+  }
+  out[s] = pos;
 }
 
 // x [B,K,C] -> out [B,C]; masked_mean semantics of utils.py:72-80.
@@ -267,6 +371,50 @@ extern "C" int se3_knn_varlen_fwd(const float* coors, const int64_t* cu_seqlens,
   knn_varlen_kernel<THREADS><<<(unsigned)total, THREADS, smem, s>>>(coors, cu_seqlens, k_per_cloud, neighbor_mask, sparse_adj,
                                                                      pair_off, num_clouds, K, valid_radius, causal, out_idx,
                                                                      out_mask, out_rel_pos, out_rel_dist);
+  SE3_LAUNCH_OK();
+  return SE3_OK;
+}
+
+extern "C" int se3_knn_csr_fwd(const float* coors, const uint8_t* node_mask, const int64_t* nbr_ptr, const int* nbr_cols,
+                               int64_t nbr_nnz, int64_t nbr_batch_stride, const int64_t* adj_ptr, const int* adj_cols,
+                               int64_t adj_nnz, int64_t adj_batch_stride, int b, int n, int k, float valid_radius, int causal,
+                               int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream) {
+  using namespace se3;
+  SE3_REQUIRE(b > 0 && n > 1, "se3_knn_csr_fwd: need b > 0 and n > 1 (got b=%d n=%d)", b, n);
+  SE3_REQUIRE(k >= 1 && k <= n - 1, "se3_knn_csr_fwd: k must be in [1, n-1] (got k=%d n=%d)", k, n);
+  SE3_REQUIRE(b <= 65535, "se3_knn_csr_fwd: b = %d exceeds the grid's y dimension (65535)", b);
+  SE3_REQUIRE(k <= KNN_TILE, "se3_knn_csr_fwd: k = %d neighbours exceeds %d, the longest list the tiled search keeps in shared memory",
+              k, KNN_TILE);
+  SE3_REQUIRE(!nbr_cols || (nbr_ptr && nbr_nnz >= 0 && (nbr_batch_stride == 0 || nbr_batch_stride == n)),
+              "se3_knn_csr_fwd: neighbour-mask rows need row pointers, nnz >= 0 and a batch stride of 0 or n");
+  SE3_REQUIRE(!adj_cols || (adj_ptr && adj_nnz >= 0 && (adj_batch_stride == 0 || adj_batch_stride == n)),
+              "se3_knn_csr_fwd: bonded rows need row pointers, nnz >= 0 and a batch stride of 0 or n");
+  constexpr int THREADS = 256;
+  const bool tiled = n - 1 > KNN_TILE;
+  const int npad = tiled ? KNN_TILE : knn_npad(n);
+  const int key_words = npad + (tiled ? next_pow2(k) : 0);
+  const size_t smem = (size_t)key_words * sizeof(unsigned long long) + 2 * CSR_BITMAP_WORDS * sizeof(unsigned);
+  if (smem > 48 * 1024)
+    SE3_CUDA_OK(cudaFuncSetAttribute(knn_csr_kernel<THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  dim3 grid(n, b);
+  knn_csr_kernel<THREADS><<<grid, THREADS, smem, as_stream(stream)>>>(coors, node_mask, nbr_ptr, nbr_cols, nbr_nnz,
+                                                                      nbr_batch_stride, adj_ptr, adj_cols, adj_nnz,
+                                                                      adj_batch_stride, n, k, npad, key_words, valid_radius,
+                                                                      causal, out_idx, out_mask, out_rel_pos, out_rel_dist);
+  SE3_LAUNCH_OK();
+  return SE3_OK;
+}
+
+extern "C" int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx,
+                                   int b, int n, int k, int64_t* out, void* stream) {
+  using namespace se3;
+  SE3_REQUIRE(b > 0 && n > 0 && k > 0 && nnz >= 0, "se3_pair_lookup_fwd: bad sizes (b=%d n=%d k=%d nnz=%lld)", b, n, k,
+              (long long)nnz);
+  SE3_REQUIRE(batch_stride == 0 || batch_stride == n, "se3_pair_lookup_fwd: batch stride must be 0 or n");
+  const int64_t total = (int64_t)b * n * k;
+  const int threads = 256;
+  pair_lookup_kernel<<<(unsigned)ceil_div(total, threads), threads, 0, as_stream(stream)>>>(row_ptr, cols, nnz, batch_stride, idx, n,
+                                                                                            k, total, out);
   SE3_LAUNCH_OK();
   return SE3_OK;
 }

@@ -27,6 +27,10 @@ def default(v, d):
     return v if exists(v) else d
 
 
+def _is_sparse(t):
+    return torch.is_tensor(t) and t.layout != torch.strided
+
+
 def to_order(degree):
     return 2 * degree + 1
 
@@ -1141,13 +1145,19 @@ class SE3Transformer(nn.Module):
         """Capture one forward for these (static) input shapes in a CUDA graph and return a replayable callable
         (see GraphedForward).  Small point clouds are launch bound (~100 kernels of a few microseconds each); replaying a
         graph removes the per-launch host cost.  Not available with attend_sparse_neighbors / neighbor_mask (their
-        host-side `.item()` synchronisations, reference S:1208, 1253, cannot be captured)."""
+        host-side `.item()` synchronisations, reference S:1208, 1253, cannot be captured), nor with sparse pair inputs."""
+        if any(_is_sparse(v) for v in fwd_kwargs.values()):
+            raise ValueError('graphed: sparse pair inputs are not supported (their number of entries is not static); pass dense '
+                             'tensors or call forward')
         return GraphedForward(self, feats, coors, mask, **fwd_kwargs)
 
     # ---- forward ----------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, feats, coors, mask=None, adj_mat=None, edges=None, return_type=None, return_pooled=False,
                 neighbor_mask=None, global_feats=None):
+        """adj_mat, edges and neighbor_mask may each also be a torch.sparse_coo tensor (see _check_sparse_pairs); the result is
+        then bit-identical to the same call with its to_dense(), and no intermediate is [n, n]."""
+        self._check_sparse_pairs(coors, adj_mat, edges, neighbor_mask)
         kw = dict(mask=mask, adj_mat=adj_mat, edges=edges, return_type=return_type, return_pooled=return_pooled,
                   neighbor_mask=neighbor_mask, global_feats=global_feats)
         return self._checked(lambda: self._forward_once(feats, coors, **kw))
@@ -1212,7 +1222,7 @@ class SE3Transformer(nn.Module):
             global_feats = {'0': global_feats[..., None]}
         if exists(global_feats):
             global_feats = {k: v.float() for k, v in global_feats.items()}
-        if exists(edges) and edges.is_floating_point():
+        if exists(edges) and edges.is_floating_point() and not edges.is_sparse:      # sparse: after coalescing, as to_dense()
             edges = edges.float()
         b, n = feats['0'].shape[:2]
         device = feats['0'].device
@@ -1220,32 +1230,33 @@ class SE3Transformer(nn.Module):
         neighbors, valid_radius = self.num_neighbors, self.valid_radius
         assert self.attend_sparse_neighbors or neighbors > 0, 'you must either attend to sparsely bonded neighbors, or set number of locally attended neighbors to be greater than 0'
 
-        adj_indices, sparse_mask, num_sparse = self._bonded(adj_mat, b, n, device)
         if neighbors == 0:
             valid_radius = 0
-        k_local = int(min(neighbors, n - 1))
-        total = int(k_local + num_sparse)
-        assert total > 0, 'you must be fetching at least 1 neighbor'
-        total = int(min(total, n - 1))
-        if exists(neighbor_mask):
-            self._report_neighbor_mask(neighbor_mask, n)
+        if any(_is_sparse(t) for t in (adj_mat, edges, neighbor_mask)):
+            idx, nmask, rel_pos, rel_dist, e = self._sparse_graph(coors, mask, adj_mat, edges, neighbor_mask, b, n, valid_radius)
+        else:
+            adj_indices, sparse_mask, num_sparse = self._bonded(adj_mat, b, n, device)
+            total = self._num_neighbors(n, num_sparse)
+            if exists(neighbor_mask):
+                eye = torch.eye(n, dtype=torch.bool, device=neighbor_mask.device)
+                self._report_neighbor_mask(neighbor_mask.masked_fill(eye.unsqueeze(0), False).sum(dim=-1))
 
-        idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=neighbor_mask,
-                                                sparse_adj=sparse_mask, causal=self.causal)
+            idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=neighbor_mask,
+                                                    sparse_adj=sparse_mask, causal=self.causal)
 
-        # edge features on the neighbour list (reference S:1231-1239, 1293-1294); gather first, embed after
-        e = None
-        if exists(edges):
-            if exists(self.edge_emb):
-                if edges.dim() == 2:                            # [b, n] tokens: the reference broadcasts them over rows (b == 1)
-                    assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
-                    edges = edges.unsqueeze(1).expand(b, n, n)
-                e = self.edge_emb(edges.gather(2, idx))
-            else:
-                e = ops.gather_pairs(edges.float(), idx)
-        if exists(self.adj_emb):
-            a = self.adj_emb(adj_indices.gather(2, idx))
-            e = torch.cat((e, a), dim=-1) if exists(e) else a
+            # edge features on the neighbour list (reference S:1231-1239, 1293-1294); gather first, embed after
+            e = None
+            if exists(edges):
+                if exists(self.edge_emb):
+                    if edges.dim() == 2:                        # [b, n] tokens: the reference broadcasts them over rows (b == 1)
+                        assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
+                        edges = edges.unsqueeze(1).expand(b, n, n)
+                    e = self.edge_emb(edges.gather(2, idx))
+                else:
+                    e = ops.gather_pairs(edges.float(), idx)
+            if exists(self.adj_emb):
+                a = self.adj_emb(adj_indices.gather(2, idx))
+                e = torch.cat((e, a), dim=-1) if exists(e) else a
 
         pos_emb = None
         if exists(self.rotary_pos_emb):
@@ -1288,7 +1299,6 @@ class SE3Transformer(nn.Module):
     def _bonded(self, adj_mat, b, n, device):
         """N-hop adjacency (reference S:1177-1191) and the bonded neighbours (S:1198-1217) of clouds of n nodes: returns
         (adj_indices [b, n, n] hop counts or None, sparse_mask [b, n, n] or None, num_sparse)."""
-        eye = torch.eye(n, dtype=torch.bool, device=device)
         max_sparse = self.max_sparse_neighbors
         adj_indices = None
         if exists(self.num_adj_degrees):                       # N-hop adjacency, reference S:1177-1191
@@ -1308,6 +1318,7 @@ class SE3Transformer(nn.Module):
             assert exists(adj_mat), 'adjacency matrix must be passed in (keyword argument adj_mat)'
             if adj_mat.dim() == 2:
                 adj_mat = adj_mat.unsqueeze(0).expand(b, -1, -1)
+            eye = torch.eye(n, dtype=torch.bool, device=device)
             adj_vals = adj_mat.float().masked_fill(eye.unsqueeze(0), 0.)
             adj_max = int(adj_vals.sum(dim=-1).max().item())
             if max_sparse < adj_max:
@@ -1322,9 +1333,152 @@ class SE3Transformer(nn.Module):
 
         return adj_indices, sparse_mask, num_sparse
 
-    def _report_neighbor_mask(self, neighbor_mask, n):
-        eye = torch.eye(n, dtype=torch.bool, device=neighbor_mask.device)
-        max_nb = int(neighbor_mask.masked_fill(eye.unsqueeze(0), False).sum(dim=-1).max().item())
+    def _num_neighbors(self, n, num_sparse):
+        """Neighbour slots per node: the local neighbours plus the bonded ones, at most n - 1 (reference S:1220-1226)."""
+        total = int(int(min(self.num_neighbors, n - 1)) + num_sparse)
+        assert total > 0, 'you must be fetching at least 1 neighbor'
+        return int(min(total, n - 1))
+
+    # ---- sparse pair inputs --------------------------------------------------------------------------------
+    def _check_sparse_pairs(self, coors, adj_mat, edges, neighbor_mask):
+        """The sparse pair inputs forward takes, checked before any device work (missing entries mean: not bonded, not
+        allowed, token 0 / a zero feature vector):
+          adj_mat        torch.sparse_coo [n, n] (shared by the batch) or [b, n, n], any real dtype;
+          neighbor_mask  torch.sparse_coo [n, n], [1, n, n] or [b, n, n], any real dtype;
+          edges          torch.sparse_coo [b, n, n] integer tokens (num_edge_tokens), or [b, n, n, edge_dim] with 3 sparse
+                         dims and 1 dense dim (continuous edges)."""
+        named = (('adj_mat', adj_mat), ('edges', edges), ('neighbor_mask', neighbor_mask))
+        if not any(_is_sparse(t) for _, t in named):
+            return
+        if not torch.is_tensor(coors) or coors.dim() != 3:
+            raise ValueError(f'coors must be [b, n, 3], got {tuple(coors.shape) if torch.is_tensor(coors) else type(coors).__name__}')
+        b, n = coors.shape[:2]
+        for name, t in named:
+            if not _is_sparse(t):
+                continue
+            if t.layout != torch.sparse_coo:
+                raise ValueError(f'{name}: the sparse layout {t.layout} is not supported; pass a torch.sparse_coo tensor '
+                                 f'({name}.to_sparse_coo())')
+            if t.dtype.is_complex:
+                raise ValueError(f'{name}: complex values are not supported, got {t.dtype}')
+            shape = tuple(t.shape)
+            if name == 'edges':
+                if t.dim() == 2:
+                    raise ValueError('edges: a 2-D sparse tensor is not accepted (it would be ambiguous with the [b, n] token '
+                                     f'form); pass [b, n, n] = {(b, n, n)}')
+                if exists(self.edge_emb):
+                    if shape != (b, n, n) or t.dense_dim() != 0:
+                        raise ValueError(f'edges: sparse edge tokens must be [b, n, n] = {(b, n, n)} with no dense dims, got '
+                                         f'{shape} with {t.dense_dim()} dense dims')
+                    if t.dtype.is_floating_point or t.dtype == torch.bool:
+                        raise ValueError(f'edges: sparse edge tokens must have an integer dtype, got {t.dtype}')
+                elif t.dim() != 4 or shape[:3] != (b, n, n) or t.sparse_dim() != 3:
+                    raise ValueError(f'edges: sparse continuous edges must be [b, n, n, edge_dim] with b, n = {(b, n)}, 3 sparse '
+                                     f'dims and 1 dense dim, got {shape} with {t.sparse_dim()} sparse dims')
+                continue
+            allowed = [(n, n), (b, n, n)] + ([(1, n, n)] if name == 'neighbor_mask' else [])
+            if shape not in allowed or t.dense_dim() != 0:
+                raise ValueError(f'{name}: a sparse {name} must be one of {sorted(set(allowed))} with no dense dims, got {shape} '
+                                 f'with {t.dense_dim()} dense dims')
+
+    def _bonded_sparse(self, adj_mat, b, n):
+        """_bonded for a torch.sparse_coo adj_mat ([n, n] or [b, n, n]) in O(nnz) memory, on the block-diagonal [R, R] matrix
+        of its clouds (R = n for a shared [n, n]).  Returns (hop counts as PairRows or None, bonded neighbours as PairRows or
+        None, num_sparse): the densified PairRows equal _bonded's adj_indices and sparse_mask, except that a random
+        sub-sample (max_sparse_neighbors below a row's bonded count) has the same distribution, not the same draw."""
+        a = ops.coo_to_rows(adj_mat, n)
+        R = a.ptr.numel() - 1
+        rows = torch.repeat_interleave(torch.arange(R, device=a.ptr.device), a.ptr.diff())
+        cols = a.cols.long() + (rows // n) * n                                             # global column of the block
+        keys, vals = rows * R + cols, a.values.float()                                     # M_1 = A, sorted by key
+        hop_keys = hop_vals = None
+        if exists(self.num_adj_degrees):
+            hop_keys, hop_vals = keys, a.values.long()
+            for degree in range(2, self.num_adj_degrees + 1):
+                m = torch.sparse_coo_tensor(torch.stack((keys // R, keys % R)), vals, (R, R), is_coalesced=True)
+                sq = torch.sparse.mm(m, m).coalesce()
+                nxt = sq.indices()[:, sq.values() > 0]
+                nxt_keys = nxt[0] * R + nxt[1]                                            # M_d = (M_{d-1} @ M_{d-1}) > 0
+                # the reference's XOR: pairs where M_d (1 or absent) differs from M_{d-1} (its value or absent) take this degree
+                pos = torch.searchsorted(keys, nxt_keys).clamp(max=max(keys.numel() - 1, 0))
+                prev = torch.where(keys[pos] == nxt_keys, vals[pos], 0.) if keys.numel() else torch.zeros_like(nxt_keys, dtype=torch.float)
+                flip = torch.cat((nxt_keys[prev != 1.], keys[(vals != 0.) & ~torch.isin(keys, nxt_keys)]))
+                keep = ~torch.isin(hop_keys, flip)
+                hop_keys, order = torch.cat((hop_keys[keep], flip)).sort()
+                hop_vals = torch.cat((hop_vals[keep], torch.full_like(flip, degree)))[order]
+                keys, vals = nxt_keys, torch.ones(nxt_keys.numel(), device=keys.device)
+        hops = None
+        if hop_keys is not None:
+            hop_rows = hop_keys // R
+            hops = ops.pair_rows(hop_rows, hop_keys % R - (hop_rows // n) * n, hop_vals, R, R == n)
+
+        bonded, num_sparse = None, 0
+        if self.attend_sparse_neighbors:                       # reference S:1198-1217 on the entries of M_D
+            rows, cols = keys // R, keys % R
+            off = rows != cols
+            rows, cols, vals = rows[off], cols[off], vals[off]
+            row_sums = torch.zeros(R, device=vals.device).index_add_(0, rows, vals)
+            adj_max = int(row_sums.max().item())
+            subsample = self.max_sparse_neighbors < adj_max
+            num_sparse = int(min(self.max_sparse_neighbors, adj_max))
+            if subsample and R == n and b > 1:                 # every cloud draws its own subset of the shared adjacency
+                shift = (torch.arange(b, device=rows.device) * n).repeat_interleave(rows.numel())
+                rows, cols, vals = rows.repeat(b) + shift, cols.repeat(b) + shift, vals.repeat(b)
+                R = b * n
+            score = vals + torch.empty_like(vals).uniform_(-0.01, 0.01) if subsample else vals
+            # the top num_sparse scores of every row (ties: lower column first), of which those above 0.5 are bonded
+            order = torch.argsort(-score, stable=True)
+            order = order[torch.argsort(rows[order], stable=True)]
+            ptr = ops.pair_rows(rows, cols, vals, R, False).ptr
+            rank = torch.arange(order.numel(), device=rows.device) - ptr[rows[order]]
+            pick = order[(rank < num_sparse) & (score[order] > 0.5)].sort().values
+            brows = rows[pick]
+            bonded = ops.pair_rows(brows, cols[pick] - (brows // n) * n, torch.ones_like(brows, dtype=torch.bool), R, R == n)
+        return hops, bonded, num_sparse
+
+    def _sparse_graph(self, coors, mask, adj_mat, edges, neighbor_mask, b, n, valid_radius):
+        """The neighbour graph and edge features of _forward_once when at least one pair input is torch.sparse_coo (the dense
+        ones are converted): the search reads sorted column lists (ops.knn_csr), and edge tokens, edge features and hop counts
+        are looked up in them (ops.pair_lookup).  Memory is O(nnz + n k).  Returns idx, nmask, rel_pos, rel_dist, e."""
+        hops, bonded, num_sparse = None, None, 0
+        if exists(self.num_adj_degrees) or self.attend_sparse_neighbors:
+            assert exists(adj_mat), 'adjacency matrix must be passed in (keyword argument adj_mat)'
+            hops, bonded, num_sparse = self._bonded_sparse(adj_mat if adj_mat.is_sparse else adj_mat.to_sparse(), b, n)
+        total = self._num_neighbors(n, num_sparse)
+        nbr = None
+        if exists(neighbor_mask):
+            nbr = ops.coo_to_rows(neighbor_mask if neighbor_mask.is_sparse else neighbor_mask.to_sparse(), n)
+            rows = torch.repeat_interleave(torch.arange(nbr.ptr.numel() - 1, device=nbr.ptr.device), nbr.ptr.diff())
+            v = nbr.values
+            off, dt = nbr.cols.long() != rows % n, v.sum().dtype                           # dt: the dtype of the dense row sums
+            self._report_neighbor_mask(torch.zeros(nbr.ptr.numel() - 1, dtype=dt, device=v.device).index_add_(0, rows[off], v[off].to(dt)))
+            allowed = v if v.dtype == torch.bool else v.to(torch.uint8) != 0              # the byte the dense search reads
+            nbr = ops.pair_rows(rows[allowed], nbr.cols[allowed], v[allowed], nbr.ptr.numel() - 1, nbr.shared)
+        idx, nmask, rel_pos, rel_dist = ops.knn_csr(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=nbr,
+                                                    bonded=bonded, causal=self.causal)
+
+        def lookup(rows):
+            """rows.values on the neighbour list, zero where a pair is absent"""
+            v = rows.values
+            return torch.cat((v, v.new_zeros((1, *v.shape[1:]))))[ops.pair_lookup(rows, idx)]
+
+        e = None
+        if exists(edges):
+            if not edges.is_sparse:
+                if exists(self.edge_emb) and edges.dim() == 2:  # [b, n] tokens: the reference broadcasts them over rows (b == 1)
+                    assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
+                    edges = edges.unsqueeze(1).expand(b, n, n)
+                edges = edges.to_sparse(3)
+            pairs = ops.coo_to_rows(edges, n)
+            e = self.edge_emb(lookup(pairs)) if exists(self.edge_emb) else lookup(pairs._replace(values=pairs.values.float()))
+        if exists(self.adj_emb):
+            a = self.adj_emb(lookup(hops))
+            e = torch.cat((e, a), dim=-1) if exists(e) else a
+        return idx, nmask, rel_pos, rel_dist, e
+
+    def _report_neighbor_mask(self, row_counts):
+        """Reference S:1253: row_counts [...] are the row sums of neighbor_mask without its diagonal."""
+        max_nb = int(row_counts.max().item())
         if max_nb > self.num_neighbors:
             print(f'neighbor_mask shows maximum number of neighbors as {max_nb} but specified number of neighbors is {self.num_neighbors}')
 
@@ -1404,6 +1558,9 @@ class SE3Transformer(nn.Module):
                                  f'{len(per_cloud) if isinstance(per_cloud, (list, tuple)) else type(per_cloud).__name__}')
             dims = 3 if name == 'edges' and not exists(self.edge_emb) else 2
             for c, (t, n) in enumerate(zip(per_cloud, seqlens)):
+                if _is_sparse(t):
+                    raise ValueError(f'forward_packed: {name}[{c}] is a sparse tensor; forward_packed takes dense per-cloud '
+                                     f'tensors (its clouds have at most {ops.MAX_CLOUD} nodes), or use forward for sparse pair inputs')
                 if not torch.is_tensor(t) or t.dim() != dims or tuple(t.shape[:2]) != (n, n):
                     want = f'[{n}, {n}, edge_dim]' if dims == 3 else f'[{n}, {n}]'
                     raise ValueError(f'forward_packed: {name}[{c}] must be {want} for a cloud of {n} nodes, got '
@@ -1449,7 +1606,8 @@ class SE3Transformer(nn.Module):
             if exists(adj_indices):
                 hops.append(adj_indices.reshape(-1))
             if exists(neighbor_mask):
-                self._report_neighbor_mask(neighbor_mask[c].to(dev).unsqueeze(0), n)
+                eye = torch.eye(n, dtype=torch.bool, device=dev)
+                self._report_neighbor_mask(neighbor_mask[c].to(dev).masked_fill(eye, False).sum(dim=-1))
         nbr = torch.cat([m.to(dev).reshape(-1) for m in neighbor_mask]) if exists(neighbor_mask) else None
         idx, nmask, rel_pos, rel_dist = ops.knn_varlen(coors.float(), seqlens, ks, max(ks), valid_radius, neighbor_mask=nbr,
                                                        sparse_adj=torch.cat(sparse) if sparse else None, causal=self.causal)

@@ -7,6 +7,7 @@ non-CUDA tensor, or without the compiled library, raises.
 import ctypes
 import os
 import threading
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -24,6 +25,9 @@ _SIGNATURES = {
     'se3_abi_version': (c_int, []),
     'se3_knn_fwd': (c_int, [c_void_p] * 4 + [c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
     'se3_knn_varlen_fwd': (c_int, [c_void_p] * 6 + [c_int, c_int64, c_int, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
+    'se3_knn_csr_fwd': (c_int, [c_void_p] * 4 + [c_int64, c_int64] + [c_void_p] * 2 + [c_int64, c_int64, c_int, c_int, c_int, c_float, c_int]
+                        + [c_void_p] * 4 + [c_void_p]),
+    'se3_pair_lookup_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
     'se3_radial_trunk_fwd': (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -168,6 +172,86 @@ def knn(coors, k, valid_radius, node_mask=None, neighbor_mask=None, sparse_adj=N
         _check(lib().se3_knn_fwd(_p(coors), _p(nm), _p(nbm), _p(sa), b, n, k, valid_radius, int(bool(causal)),
                                  _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
     return idx, mask.view(torch.bool), rel_pos, rel_dist
+
+
+class PairRows(NamedTuple):
+    """A sparse pair input in the row format of se3_knn_csr_fwd: row r = b * n + i (or i when shared) holds entries
+    ptr[r] .. ptr[r+1] of cols (ascending, unique) and values."""
+    ptr: torch.Tensor         # int64 [rows + 1]
+    cols: torch.Tensor        # int32 [nnz], node index inside the cloud
+    values: torch.Tensor      # [nnz, ...] in the input's dtype
+    shared: bool              # one [n, n] list for every cloud of the batch (batch stride 0)
+
+
+def pair_rows(rows, cols, values, num_rows, shared):
+    """PairRows from entries sorted by (row, col): rows int64 [nnz] in [0, num_rows), cols [nnz]."""
+    ptr = torch.zeros(num_rows + 1, dtype=torch.int64, device=rows.device)
+    ptr[1:] = torch.bincount(rows, minlength=num_rows).cumsum(0)
+    return PairRows(ptr, cols.to(torch.int32), values, shared)
+
+
+def coo_to_rows(t, n):
+    """A torch.sparse_coo pair input [n, n] or [B, n, n] (sparse dims; dense dims after them stay in the values) -> PairRows.
+    Coalescing sums duplicate entries, as to_dense() does; stored zeros and diagonal entries are kept.  [n, n] and [1, n, n]
+    give one shared list.  Torch only, so it also runs on the CPU."""
+    t = t.coalesce()
+    ind = t.indices()
+    if t.sparse_dim() == 2:
+        rows, cols, B = ind[0], ind[1], 1
+    else:
+        rows, cols, B = ind[0] * n + ind[1], ind[2], t.shape[0]
+    return pair_rows(rows, cols, t.values(), B * n, B == 1)
+
+
+def _row_args(rows, b, n):
+    """(ptr, cols, nnz, batch stride) of a PairRows for a batch [b, n]; an empty list keeps a non-NULL column pointer, since
+    NULL means no list."""
+    if rows is None:
+        return None, None, 0, 0
+    want = (n if rows.shared else b * n) + 1
+    if rows.ptr.dtype != torch.int64 or rows.ptr.shape != (want,) or rows.cols.dtype != torch.int32 or rows.cols.dim() != 1:
+        raise ValueError(f'pair rows for b, n = {(b, n)} need int64 row pointers [{want}] and int32 columns [nnz], got '
+                         f'{rows.ptr.dtype} {tuple(rows.ptr.shape)} and {rows.cols.dtype} {tuple(rows.cols.shape)}')
+    cols = rows.cols.contiguous() if rows.cols.numel() else torch.zeros(1, dtype=torch.int32, device=rows.cols.device)
+    return rows.ptr.contiguous(), cols, rows.cols.numel(), 0 if rows.shared else n
+
+
+def knn_csr(coors, k, valid_radius, node_mask=None, neighbor_mask=None, bonded=None, causal=False):
+    """knn() with the pair masks given as PairRows: neighbor_mask lists the allowed columns of each row, bonded the bonded
+    ones.  Bit-identical to knn() on the densified masks.  Returns idx int64 [b,n,k], mask bool [b,n,k], rel_pos [b,n,k,3],
+    rel_dist [b,n,k]."""
+    _require_cuda(coors, node_mask, *(r.ptr for r in (neighbor_mask, bonded) if r is not None),
+                  *(r.cols for r in (neighbor_mask, bonded) if r is not None))
+    coors = _f32(coors)
+    b, n, _ = coors.shape
+    if node_mask is not None and node_mask.shape != (b, n):
+        raise ValueError(f'knn_csr: node_mask must be [b, n] = {(b, n)}, got {tuple(node_mask.shape)}')
+    nptr, ncols, nnnz, nstride = _row_args(neighbor_mask, b, n)
+    aptr, acols, annz, astride = _row_args(bonded, b, n)
+    idx = torch.empty((b, n, k), dtype=torch.int64, device=coors.device)
+    mask = torch.empty((b, n, k), dtype=torch.uint8, device=coors.device)
+    rel_pos = torch.empty((b, n, k, 3), dtype=torch.float32, device=coors.device)
+    rel_dist = torch.empty((b, n, k), dtype=torch.float32, device=coors.device)
+    nm = _u8(node_mask)
+    valid_radius = float(min(valid_radius, 3.0e38))
+    nbytes = 12 * b * n + 25 * b * n * k + (0 if nm is None else nm.numel()) + 4 * (nnnz + annz)
+    with torch.cuda.device(coors.device), _timed('knn', nbytes=nbytes):
+        _check(lib().se3_knn_csr_fwd(_p(coors), _p(nm), _p(nptr), _p(ncols), nnnz, nstride, _p(aptr), _p(acols), annz, astride,
+                                     b, n, k, valid_radius, int(bool(causal)), _p(idx), _p(mask), _p(rel_pos), _p(rel_dist),
+                                     _stream()))
+    return idx, mask.view(torch.bool), rel_pos, rel_dist
+
+
+def pair_lookup(rows, idx):
+    """Position of every neighbour idx [b, n, k] in the PairRows rows (int64 [b, n, k]), -1 where its row lacks the pair:
+    rows.values indexed with a zero row appended for -1 are the pair values on the neighbour list."""
+    _require_cuda(idx, rows.ptr, rows.cols)
+    b, n, k = idx.shape
+    ptr, cols, nnz, stride = _row_args(rows, b, n)
+    out = torch.empty((b, n, k), dtype=torch.int64, device=idx.device)
+    with torch.cuda.device(idx.device), _timed('pair_lookup', nbytes=16 * b * n * k):
+        _check(lib().se3_pair_lookup_fwd(_p(ptr), _p(cols), nnz, stride, _p(idx.contiguous()), b, n, k, _p(out), _stream()))
+    return out
 
 
 MAX_CLOUD = 4097      # nodes per cloud of the shared-memory sort (n - 1 <= 4096 columns)
