@@ -106,23 +106,42 @@ attn_kernel(AttnArgs a) {
 // rotation back to the global frame (S:237-254 re-associated) happens here, on the fly: the query is rotated INTO the frame of
 // every edge for the logit (sum_{d,m} q k = sum_{d,n} (D^T q)[d,n] kp[n,d]) and every value is rotated out before it is
 // accumulated, so the global-frame K / V tensors are never written or read.  Prefix keys (global / null / self) are node level
-// and already in the global frame.  One warp per (node, head); lanes over dim_head; D of the node's K edges in shared memory.
-template <int P, int ND>
+// and already in the global frame.  One warp per (node, head); lanes over dim_head.  The D of the node's edges sit in shared
+// memory: all K of them when K <= kAttnEdgeTile, else (kTiled) tiles of kAttnEdgeTile edges staged in turn by the whole block,
+// so that only the logits grow with K.  In the tiled kernel a warp past the last head computes that head again and stores
+// nothing, so that every warp reaches every block barrier.  kTiled is a template switch because block barriers inside the key
+// loops cost registers.
+constexpr int kAttnEdgeTile = 32;
+
+// D of edges e0 .. e0 + te - 1 (at most K - e0) of this node into sD, by the whole block
+template <int P>
+__device__ __forceinline__ void stage_frames(float* sD, const float* __restrict__ Dmat, int64_t node, int K, int e0, int te, bool sync_before) {
+  if (sync_before) __syncthreads();                           // every warp is done with the previous tile
+  const int cnt = min(te, K - e0) * P * P;
+  const float* src = Dmat + ((size_t)node * K + e0) * P * P;
+  for (int t = threadIdx.x; t < cnt; t += blockDim.x) sD[t] = src[t];
+  __syncthreads();
+}
+
+template <int P, int ND, bool kTiled>
 __global__ void __launch_bounds__(kAttnWarps * 32)
 attn_aligned_kernel(AttnArgs a, const float* __restrict__ Dmat, int k_aligned) {
   extern __shared__ float smem_dyn[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t node = (int64_t)blockIdx.x;
-  const int h = blockIdx.y * kAttnWarps + warp;
+  const int h_warp = blockIdx.y * kAttnWarps + warp;
+  const int h = min(h_warp, a.H - 1);
   const int64_t bb = node / a.n, i = node % a.n;
   const int Ckv = a.kv_heads * a.Dh;
   const int prefix = a.G + a.has_null + a.has_self;
   const int J = prefix + a.K;
-  float* sD = smem_dyn;                                       // [K][P*P]
-  float* logits = smem_dyn + (size_t)a.K * P * P + (size_t)warp * J;
-  for (int t = threadIdx.x; t < a.K * P * P; t += blockDim.x) sD[t] = Dmat[(size_t)node * a.K * P * P + t];
-  __syncthreads();
-  if (h >= a.H) return;
+  const int te = kTiled ? kAttnEdgeTile : a.K;
+  float* sD = smem_dyn;                                       // [te][P*P]: D of edges t0 .. t0 + te - 1
+  float* logits = smem_dyn + (size_t)te * P * P + (size_t)warp * J;
+  if (!kTiled) {
+    stage_frames<P>(sD, Dmat, node, a.K, 0, te, false);
+    if (h_warp >= a.H) return;                                // no block barrier follows
+  }
   const int hk = a.kv_heads == 1 ? 0 : h;
   const int L = a.Dh * P;
 
@@ -134,7 +153,9 @@ attn_aligned_kernel(AttnArgs a, const float* __restrict__ Dmat, int k_aligned) {
     for (int m = 0; m < P; ++m) qv[t][m] = (d < a.Dh) ? a.q[((size_t)node * a.H + h) * L + (size_t)d * P + m] : 0.f;
   }
   const uint8_t* mrow = a.nmask ? a.nmask + (size_t)node * a.K : nullptr;
-  for (int j = 0; j < J; ++j) {
+  for (int j = 0, t0 = kTiled ? -te : 0; j < J; ++j) {
+    const int jj = j - prefix;
+    if (kTiled && k_aligned && jj == t0 + te) { t0 = jj; stage_frames<P>(sD, Dmat, node, a.K, t0, te, t0 > 0); }
     float s = 0.f;
     if (j < prefix || !k_aligned) {
       const float* kp = kv_ptr(a, true, bb, i, j, hk, L, Ckv);
@@ -147,9 +168,8 @@ attn_aligned_kernel(AttnArgs a, const float* __restrict__ Dmat, int k_aligned) {
         }
       }
     } else {
-      const int jj = j - prefix;
       if (mrow == nullptr || mrow[jj]) {
-        const float* dm = sD + jj * P * P;
+        const float* dm = sD + (jj - t0) * P * P;
         const float* kp = a.k + (((size_t)node * a.K + jj) * P) * Ckv + (size_t)hk * a.Dh;
 #pragma unroll
         for (int t = 0; t < ND; ++t) {
@@ -185,7 +205,9 @@ attn_aligned_kernel(AttnArgs a, const float* __restrict__ Dmat, int k_aligned) {
   for (int t = 0; t < ND; ++t)
 #pragma unroll
     for (int m = 0; m < P; ++m) acc[t][m] = 0.f;
-  for (int j = 0; j < J; ++j) {
+  for (int j = 0, t0 = kTiled ? -te : 0; j < J; ++j) {
+    const int jj = j - prefix;
+    if (kTiled && jj == t0 + te) { t0 = jj; stage_frames<P>(sD, Dmat, node, a.K, t0, te, true); }
     const float aj = logits[j] * inv;
     if (j < prefix) {
       const float* vp = kv_ptr(a, false, bb, i, j, hk, L, Ckv);
@@ -198,9 +220,8 @@ attn_aligned_kernel(AttnArgs a, const float* __restrict__ Dmat, int k_aligned) {
         }
       }
     } else {
-      const int jj = j - prefix;
       if (aj == 0.f) continue;                                  // masked neighbour (warp uniform)
-      const float* dm = sD + jj * P * P;
+      const float* dm = sD + (jj - t0) * P * P;
       const float* vp = a.v + (((size_t)node * a.K + jj) * P) * Ckv + (size_t)hk * a.Dh;
 #pragma unroll
       for (int t = 0; t < ND; ++t) {
@@ -220,6 +241,7 @@ attn_aligned_kernel(AttnArgs a, const float* __restrict__ Dmat, int k_aligned) {
       }
     }
   }
+  if (h_warp >= a.H) return;
 #pragma unroll
   for (int t = 0; t < ND; ++t) {
     const int d = lane + 32 * t;
@@ -233,16 +255,21 @@ attn_aligned_kernel(AttnArgs a, const float* __restrict__ Dmat, int k_aligned) {
 template <int P>
 static int launch_attn_aligned(const AttnArgs& a, const float* D, int k_aligned, cudaStream_t s) {
   const int J = a.G + a.has_null + a.has_self + a.K;
-  const size_t smem = ((size_t)a.K * P * P + (size_t)kAttnWarps * J) * sizeof(float);
+  const bool tiled = a.K > kAttnEdgeTile;
+  const int te = tiled ? kAttnEdgeTile : a.K;
+  const size_t smem = ((size_t)te * P * P + (size_t)kAttnWarps * J) * sizeof(float);
   SE3_REQUIRE(smem <= 200 * 1024, "se3_attn_aligned_fwd: %d keys per query exceed the shared-memory budget", J);
   dim3 grid((unsigned)((int64_t)a.b * a.n), (unsigned)ceil_div(a.H, kAttnWarps));
+  const int warps = min(a.H, kAttnWarps);                     // (fewer than kAttnWarps heads: no idle warps)
   const int ND = (int)ceil_div(a.Dh, 32);
-#define SE3_AA(NDV)                                                                                                          \
+#define SE3_AA_T(NDV, TILED)                                                                                                 \
   {                                                                                                                          \
-    if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(attn_aligned_kernel<P, NDV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    attn_aligned_kernel<P, NDV><<<grid, kAttnWarps * 32, smem, s>>>(a, D, k_aligned);                                        \
+    if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(attn_aligned_kernel<P, NDV, TILED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    attn_aligned_kernel<P, NDV, TILED><<<grid, warps * 32, smem, s>>>(a, D, k_aligned);                                      \
   }
+#define SE3_AA(NDV) { if (tiled) SE3_AA_T(NDV, true) else SE3_AA_T(NDV, false) }
   if (ND <= 1) SE3_AA(1) else if (ND <= 2) SE3_AA(2) else SE3_AA(4)
+#undef SE3_AA_T
 #undef SE3_AA
   SE3_LAUNCH_OK();
   return SE3_OK;

@@ -916,7 +916,8 @@ class AttentionSE3(nn.Module):
         queries = self.to_q(features)
         k_idx = None
         geom = basis[2] if isinstance(basis, tuple) and len(basis) > 2 else None
-        fuse = geom is not None and not switches.current().no_attn_rotate    # rotate-back fused into the attention kernel
+        # rotate-back fused into the attention kernel
+        fuse = geom is not None and not switches.current().no_attn_rotate and ops.attn_aligned_supported(self.dim_head)
         if self.linear_proj_keys:
             values = conv_forward([self.to_v], features, edge_info, rel_dist, basis, keep_aligned=fuse)[0]
             keys = self.to_k(features)            # node level; the attention kernel gathers through idx

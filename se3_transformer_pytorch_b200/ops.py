@@ -843,6 +843,14 @@ def pool(x, mask):
 # ---------------------------------------------------------------------------------------------------------
 # K5
 # ---------------------------------------------------------------------------------------------------------
+ATTN_ALIGNED_MAX_DIM_HEAD = 128     # se3_attn_aligned_fwd keeps dim_head in at most 4 register slots per lane
+
+
+def attn_aligned_supported(dim_head):
+    """Heads the attention kernel with the fused rotate-back takes; wider heads rotate back separately and run se3_attn_fwd."""
+    return dim_head <= ATTN_ALIGNED_MAX_DIM_HEAD
+
+
 def attention(q, k, v, *, heads, dim_head, scale, nmask=None, k_idx=None, self_k=None, self_v=None, null_k=None, null_v=None,
               global_k=None, global_v=None, kv_heads=None, D=None, k_aligned=False):
     """One degree of AttentionSE3 / OneHeadedKVAttentionSE3 (reference S:476-517, 612-652).

@@ -8,7 +8,8 @@ Outputs
   tests/golden/sh_basis.npz                         Y_J + get_basis on fixed vectors (basis.py:140-205)
   tests/golden/model_<case>.npz                     whole-model inputs/outputs + captured intermediates (largest arrays
                                                     in model_<case>.part<i>.npz, so that every file stays under 1 MB)
-  tests/golden/state_keys.json                      state_dict key/shape lists (SURVEY.md A.6)
+  tests/golden/state_keys.json                      state_dict key/shape lists (SURVEY.md A.6); the DEG_CASES fixtures
+                                                    hold their own as 'state_keys'
 
 Weights are never stored: both sides fill state_dict() with tests/golden/detfill.py.
 """
@@ -144,6 +145,20 @@ RCASES = [
 ]
 
 
+# the top of the documented degree range (num_degrees 5 and 6: Q_J tables and kernel templates up to degree 5).  tc_deg5 puts
+# the tensor-core kernels on pairs with degree_in = 4 and SIMT on degree_out = 4; z128_deg6 runs the attention convolutions on
+# the mixed low-rank / SIMT route and conv_out (outputs of degree <= 1) on the one-GEMM path with inputs up to degree 5.
+# These models have ~1000 parameter tensors each: their state_dict layout is stored in the fixture ('state_keys'), not in
+# state_keys.json.
+DEG_CASES = [
+    dict(name='deg6', ctor=dict(dim=16, heads=2, dim_head=8, depth=1, num_degrees=6, output_degrees=2, num_neighbors=4), b=1, n=10,
+         capture_kv=True),
+    dict(name='tc_deg5', ctor=dict(dim=32, heads=2, dim_head=16, depth=1, num_degrees=5, output_degrees=2, num_neighbors=6), b=1, n=16),
+    dict(name='z128_deg6', ctor=dict(dim=128, heads=2, dim_head=64, depth=1, num_degrees=6, output_degrees=2, num_neighbors=4), b=1, n=8,
+         no_capture=True),
+]
+
+
 def build_inputs(case):
     b, n = case['b'], case['n']
     name = case['name']
@@ -269,9 +284,11 @@ def run_case(case):
         out['cap/' + k] = v
     out['config'] = np.array(json.dumps(dict(ctor={k: (list(v) if isinstance(v, tuple) else v) for k, v in case['ctor'].items()},
                                              fwd=case.get('fwd', {}), b=case['b'], n=case['n'])))
+    keys = {k: list(v.shape) for k, v in model.state_dict().items()}
+    if name in {c['name'] for c in DEG_CASES}:
+        out['state_keys'] = np.array(json.dumps(keys, sort_keys=True))
     path = os.path.join(HERE, f'model_{name}.npz')
     write_split(path, out)
-    keys = {k: list(v.shape) for k, v in model.state_dict().items()}
     print('wrote', path, 'params', sum(int(np.prod(s)) for s in keys.values()), 'size', os.path.getsize(path))
     return keys
 
@@ -288,7 +305,7 @@ def write_split(path, arrays, limit=900_000):
     for k in sorted(main, key=lambda k: -main[k].nbytes):
         if size(main) <= limit:
             break
-        if k == 'config':
+        if k in ('config', 'state_keys'):
             continue
         if parts and size({**parts[-1], k: main[k]}) <= limit:
             parts[-1][k] = main.pop(k)
@@ -313,6 +330,9 @@ if __name__ == '__main__':
         gen_sh_basis()
     if 'rot' in which:
         gen_equivariance_inputs()
+    if 'deg' in which:
+        for case in DEG_CASES:
+            run_case(case)
     if 'models' in which or 'big' in which or 'z' in which or 'rotary' in which:
         kpath = os.path.join(HERE, 'state_keys.json')
         all_keys = json.load(open(kpath)) if os.path.exists(kpath) else {}

@@ -16,6 +16,9 @@ BIG_CASES = ['cfg3', 'cfg4_b2']
 # widths the one-GEMM production kernel takes (every fiber a multiple of 128 channels, DESIGN.md 4.5)
 Z_CASES = ['z128', 'z256_deg4']
 
+# num_degrees 5 and 6, the top of the documented range (tests/golden/gen_golden.py DEG_CASES)
+DEG_CASES = ['deg6', 'tc_deg5', 'z128_deg6']
+
 
 def load_case(name):
     z = dict(np.load(os.path.join(GOLDEN, f'model_{name}.npz')))
@@ -31,7 +34,10 @@ def load_case(name):
 
 def state_keys(name):
     with open(os.path.join(GOLDEN, 'state_keys.json')) as f:
-        return json.load(f)[name]
+        keys = json.load(f)
+    if name in keys:
+        return keys[name]
+    return json.loads(str(load_case(name)[0]['state_keys']))      # (DEG_CASES: stored in the fixture)
 
 
 def det_params(name, seed=11):

@@ -6,7 +6,7 @@ import re
 import pytest
 import torch
 
-from helpers import MODEL_CASES, BIG_CASES, Z_CASES, load_case, state_keys
+from helpers import MODEL_CASES, BIG_CASES, Z_CASES, DEG_CASES, load_case, state_keys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -19,6 +19,12 @@ def test_state_dict_layout_matches_reference(name):
     model = SE3Transformer(**cfg['ctor'])
     mine = {k: list(v.shape) for k, v in model.state_dict().items()}
     assert mine == state_keys(name)
+
+
+@pytest.mark.parametrize('name', DEG_CASES)
+def test_state_dict_layout_matches_reference_high_degree(name):
+    """The same at 5 and 6 degrees."""
+    test_state_dict_layout_matches_reference(name)
 
 
 def test_library_matches_header_at_abi_version_2():
