@@ -10,6 +10,7 @@ Forward only: everything runs under torch.no_grad().  CUDA only: there is no CPU
 """
 import operator
 from math import sqrt
+from typing import NamedTuple
 
 import torch
 import torch.nn.functional as F
@@ -218,7 +219,9 @@ class ConvSE3(nn.Module):
         self.self_interaction = self_interaction
         self.num_fourier_features = num_fourier_features
         self.fourier_encode_dist = fourier_encode_dist
-        self.splits = splits          # accepted for API parity; chunking is by T_WORKSPACE_BYTES instead
+        # accepted for API parity and ignored: SE3Transformer evaluates the edge work of every block over node chunks sized by
+        # the edge_budget_mb switch (SE3B200_EDGE_BUDGET_MB, plan_node_chunks) instead of a fixed number of splits
+        self.splits = splits
         edge_dim += 0 if not fourier_encode_dist else num_fourier_features * 2
         self.in_dim = edge_dim + 1
         self.kernel_unary = nn.ModuleDict()
@@ -477,7 +480,25 @@ class ConvSE3(nn.Module):
         return feat.reshape(-1, feat.shape[-1]).contiguous()
 
     def forward(self, inp, edge_info, rel_dist=None, basis=None):
-        return conv_forward([self], inp, edge_info, rel_dist, basis)[0]
+        geom = basis[2] if isinstance(basis, tuple) and len(basis) > 2 else None
+        if not self.pool or geom is None or geom.edge_budget is None:
+            return conv_forward([self], inp, edge_info, rel_dist, basis)[0]
+        # node chunks under the edge budget: the pooled outputs of every chunk land in their rows of the node-level result
+        decisions = [conv_decide(self, edge_info[0].numel(), rel_dist, geom, torch.cuda.is_current_stream_capturing())]
+        chunks = geom.node_chunks(decisions, edge_info[0].shape)
+        if len(chunks) == 1:
+            return conv_forward([self], inp, edge_info, rel_dist, basis, decisions=decisions)[0]
+        self_out = self.self_interact(inp) if self.self_interaction else None
+        sx = chunk_edge_scale(decisions, inp, edge_info[0])
+        b, n = edge_info[0].shape[:2]
+        out = {str(do): torch.empty((b, n, mo, to_order(do)), dtype=torch.float32, device=rel_dist.device)
+               for do, mo in self.fiber_out}
+        for c in chunks:
+            res = conv_forward([self], c.src(inp), c.edge_info(edge_info), c.rows(rel_dist), (None, None, geom.chunk(c)),
+                               decisions=decisions, self_out=c.rows(self_out), sx=c.rows(sx))[0]
+            for d, t in res.items():
+                c.rows(out[d]).copy_(t)
+        return out
 
 
 def input_side(di, do):
@@ -493,21 +514,45 @@ def lowrank_k(r):
 
 
 class Geometry:
-    """Per-forward edge geometry shared by every layer; the aligned frames are built on first use, by the code that the
-    host_frames switch selects when the Geometry is made."""
+    """Per-forward edge geometry shared by every layer; the aligned frames and the flat basis are built on first use, the frames
+    by the code that the host_frames switch selects when the Geometry is made.  chunk() gives the Geometry of the edges of one
+    node chunk (NodeChunk), which builds its own frames and basis and shares the whole graph's d_max and deferred checks."""
 
-    def __init__(self, rel_pos, max_degree):
-        self.rel_pos, self.max_degree, self._frames = rel_pos, max_degree, None
-        self.host_frames = switches.current().host_frames
+    def __init__(self, rel_pos, max_degree, whole=None):
+        self.rel_pos, self.max_degree, self._frames, self._basis = rel_pos, max_degree, None, None
+        self.whole = self if whole is None else whole
+        self.host_frames = switches.current().host_frames if whole is None else whole.host_frames
         # run-time checks of the low-rank plans, as (ConvSE3, stats [pairs, 2]) : None = check inside every ConvSE3 (one host
         # synchronisation each); a list = the caller collects them and checks once per forward (SE3Transformer.forward)
-        self.deferred = None
+        self.deferred = None if whole is None else whole.deferred
         self._dmax = None
+        # bytes the edge-level tensors of one block may take (edge_budget_bytes), or None: every block runs as one chunk
+        self.edge_budget = None
 
     def d_max(self, rel_dist):
+        if self is not self.whole:
+            return self.whole.d_max(rel_dist)
         if self._dmax is None:
             self._dmax = float(rel_dist.max())          # the one host synchronisation of the plan lookup, once per forward
         return self._dmax
+
+    def chunk(self, c):
+        """The Geometry of the edges of node chunk c (self when c is the whole graph)."""
+        if c.whole:
+            return self
+        return Geometry(c.rows(self.rel_pos), self.max_degree, whole=self)
+
+    def node_chunks(self, decisions, shape, keep_aligned=False, attn_bytes=0):
+        """The node chunks of one block of the graph idx [b, n, k] = shape: one chunk without an edge budget."""
+        b, n, k = shape
+        per_edge = block_edge_bytes(decisions, self.max_degree, keep_aligned, attn_bytes)
+        return plan_node_chunks(b, n, k, per_edge, self.whole.edge_budget)
+
+    def basis(self):
+        """(flat basis buffer, BasisPlan) of these edges (ops.basis_flat), for the R-first route."""
+        if self._basis is None:
+            self._basis = ops.basis_flat(self.rel_pos, self.max_degree)
+        return self._basis
 
     def to_global(self, akv):
         """AlignedKV -> [b, n, k, C, 2lo+1] in the global frame (the rotate-back the attention kernel otherwise fuses)."""
@@ -569,6 +614,110 @@ def edge_chunks(E, tile_bytes):
         yield t0, tc, e0, min(E - e0, tc * ops.TILE_E)
 
 
+# ---- node chunks under the edge budget (DESIGN.md 4.7) -------------------------------------------------------------------
+EDGE_BUDGET_FRACTION = 0.25      # default edge budget: this share of the device's total memory, per block
+
+
+def edge_budget_bytes(sw, device):
+    """The edge budget of a forward on `device` under the switches sw: edge_budget_mb MiB if set, else EDGE_BUDGET_FRACTION of
+    the device's total (not free) memory, so that the chunking does not depend on what else is allocated."""
+    if sw.edge_budget_mb is not None:
+        return max(0, int(sw.edge_budget_mb * 2 ** 20))
+    return int(torch.cuda.get_device_properties(device).total_memory * EDGE_BUDGET_FRACTION)
+
+
+class NodeChunk(NamedTuple):
+    """Nodes n0 .. n1 of batch rows b0 .. b1: whole rows (n0, n1 = 0, n) or a range inside one row (b1 = b0 + 1).  Its edges
+    are one contiguous range of the [b, n, k] layout, whole neighbour lists only."""
+    b0: int
+    b1: int
+    n0: int
+    n1: int
+    whole: bool = False            # the chunk is the whole graph
+
+    def rows(self, t):
+        """The chunk's rows of a [b, n, ...] tensor (node or edge level), or of every tensor of a dict; None stays None."""
+        if t is None:
+            return None
+        if isinstance(t, dict):
+            return {key: self.rows(v) for key, v in t.items()}
+        return t[self.b0:self.b1, self.n0:self.n1]
+
+    def src(self, t):
+        """The node features [b, n, ...] that the chunk's neighbours are gathered from, as the kernels see them: a [b', n', ...]
+        view that starts at the chunk's first batch row.  The kernels address a neighbour as (batch row of the edge) * n' + idx
+        and a range inside one row has b' = 1, so every neighbour idx < n of that row lies inside the row's storage."""
+        if isinstance(t, dict):
+            return {key: self.src(v) for key, v in t.items()}
+        return t[self.b0:self.b1, :self.n1 - self.n0]
+
+    def edge_info(self, edge_info):
+        return tuple(self.rows(t) for t in edge_info)
+
+
+def plan_node_chunks(b, n, k, edge_bytes, budget):
+    """Node chunks (NodeChunk) of a graph of b x n nodes with k neighbours each whose edges, at edge_bytes per edge, fit
+    `budget` bytes: one chunk if the whole graph fits (or budget is None), else runs of whole batch rows, else ranges of nodes
+    inside each row.  Chunks cover every node once, in order, and are balanced; the smallest is one node, whatever its size."""
+    if budget is None or b * n * k * edge_bytes <= budget:
+        return [NodeChunk(0, b, 0, n, whole=True)]
+    cap = max(1, budget // max(1, k * edge_bytes))               # nodes per chunk
+    if cap >= n:
+        count = -(-b // (cap // n))
+        rows = -(-b // count)
+        return [NodeChunk(b0, min(b0 + rows, b), 0, n) for b0 in range(0, b, rows)]
+    count = -(-n // cap)
+    size = -(-n // count)
+    return [NodeChunk(r, r + 1, n0, min(n0 + size, n)) for r in range(b) for n0 in range(0, n, size)]
+
+
+def block_edge_bytes(decisions, max_degree, keep_aligned=False, attn_bytes=0):
+    """Bytes per edge of the edge-level tensors that one node chunk of a block (the convolutions of `decisions`, which share
+    inputs and graph) holds at its peak, from the fibers and routes: edge features, frames, flat basis, radial coordinates,
+    outputs and the transient gathers / T blocks / out' of one edge chunk, plus attn_bytes of the attention glue.  An estimate."""
+    c0 = decisions[0].conv
+    fin, fout = c0.fiber_in, c0.fiber_out
+    routes = {d.route for d in decisions}
+    total = 4 * c0.in_dim + attn_bytes
+    if routes & {'production', 'aligned'} or keep_aligned:
+        total += 4 * sum(to_order(l) ** 2 for l in range(1, max_degree + 1))                          # frames D_l
+    if 'production' in routes:
+        total += 4 + 4 * sum(mi * to_order(di) for di, mi in fin) + 4 * max(mo * to_order(do) for do, mo in fout)   # sx, X, out'
+    if routes & {'aligned', 'rfirst'}:
+        total += max(ops.t_numel(1, mi, to_order(min(di, do)), to_order(do)) * 4 for di, mi in fin for do, _ in fout) // ops.TILE_E
+    if 'rfirst' in routes:
+        L = range(max_degree + 1)
+        total += 4 * sum(to_order(do) * to_order(di) * to_order(min(di, do)) for di in L for do in L)   # flat basis
+        total += 4 * max(to_order(min(di, do)) * mo * to_order(di) + mi * to_order(di) for di, mi in fin for do, mo in fout)
+    for d in decisions:
+        pairs = len(d.conv.pairs)
+        total += 4 * 64 * pairs * bool(d.lr) + 4 * ops.RADIAL_MID * pairs * d.direct             # U, g
+        if not (d.route == 'production' and d.conv.pool):
+            total += 4 * sum(mo * to_order(do) for do, mo in fout)                                 # outputs
+    return total
+
+
+def chunk_edge_scale(decisions, inp, idx):
+    """The production route's per-edge scale (ops.edge_scale) of the whole graph as [b, n, k], for the node chunks to slice: its
+    node maxima cover every row, which a chunk's view of the features does not.  None if no convolution takes that route."""
+    if not any(d.route == 'production' for d in decisions):
+        return None
+    return ops.edge_scale(inp, idx, max(di for di, _ in decisions[0].conv.fiber_in)).view(idx.shape)
+
+
+class ConvDecision:
+    """What one ConvSE3 decides once per forward, from the whole graph (conv_decide): the switches sw, tc_ok {pair: bool}, the
+    low-rank plan or None, its covered pairs lr and the route they give, whether direct kernels need g, and the stats
+    [pairs, 2] that the radial launches of every chunk accumulate into; deferred: the check is queued on Geometry.deferred."""
+
+    def __init__(self, conv, sw, tc_ok, plan, stats, deferred):
+        self.conv, self.sw, self.tc_ok, self.plan, self.stats, self.deferred = conv, sw, tc_ok, plan, stats, deferred
+        self.lr = dict(plan['pairs']) if plan is not None else {}
+        kinds = {pp['kind'] for pp in self.lr.values()}
+        self.route = 'production' if 'z' in kinds else 'aligned' if 'aligned' in kinds else 'rfirst'
+        self.direct = self.route == 'rfirst' and len(self.lr) < len(conv.pairs)
+
+
 class ConvDispatch:
     """How one ConvSE3 runs in one forward (conv_dispatch).  route: 'production' (DESIGN.md 4.5, GEMM images z), 'aligned' (4.4)
     or 'rfirst' (4.1-4.3, with each pair's kernel in how: 'input_side', 'combined', 'tc' or 'simt').  U [pairs, E, 64]: radial
@@ -597,30 +746,43 @@ def _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing):
     return None
 
 
-def conv_dispatch(conv, edge_info, rel_dist, geom, capturing):
-    """Choose the route of `conv` for this forward and launch its radial kernels (U of the low-rank pairs from the plan's table
-    or the trunk, g for the direct kernels).  The plan is checked here, or the check is queued on geom.deferred."""
+def conv_decide(conv, E, rel_dist, geom, capturing):
+    """The per-forward half of conv_dispatch, from the whole graph (E edges, distances rel_dist): the switches, tc_ok and the
+    low-rank plan, which therefore stay the same in every node chunk.  A plan's run-time check is queued on geom.deferred
+    here, once, over stats that the radial launches of all chunks accumulate into; without a deferred list conv_dispatch
+    checks it after its launches."""
+    sw = switches.current()
+    tc_ok = {pair: conv.tc_eligible(*pair) for pair in conv.pairs}
+    plan = _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing)
+    if plan is None or not plan['pairs']:
+        return ConvDecision(conv, sw, tc_ok, None, None, False)
+    stats = torch.zeros((len(conv.pairs), 2), dtype=torch.float32, device=rel_dist.device)
+    deferred = geom is not None and geom.deferred is not None
+    if deferred:
+        geom.deferred.append((conv, stats, plan['have']))          # checked once per forward by the caller
+    return ConvDecision(conv, sw, tc_ok, plan, stats, deferred)
+
+
+def conv_dispatch(conv, edge_info, rel_dist, geom, capturing, decision=None):
+    """Launch the radial kernels of `conv` on these edges (U of the low-rank pairs from the plan's table or the trunk, g for the
+    direct kernels) under `decision` (conv_decide on these edges if None), and set up its outputs."""
     idx = edge_info[0]
     E, dev = idx.numel(), idx.device
-    sw = switches.current()
+    d = conv_decide(conv, E, rel_dist, geom, capturing) if decision is None else decision
+    sw, tc_ok, plan = d.sw, d.tc_ok, d.plan
     pk = conv.packed(sw)
     feat = conv.edge_features(edge_info, rel_dist)
     assert feat.shape[-1] == conv.in_dim, f'edge feature width {feat.shape[-1]} != {conv.in_dim}'
-    tc_ok = {pair: conv.tc_eligible(*pair) for pair in conv.pairs}
-    plan = _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing)
     lr, U, g, route = {}, None, None, 'rfirst'
-    if plan is not None and plan['pairs']:
+    if plan is not None:
         covered = len(plan['pairs']) == len(conv.pairs)
-        stats = torch.zeros((len(conv.pairs), 2), dtype=torch.float32, device=dev)
+        stats = d.stats
         if covered and plan['utab'] is not None and not sw.no_utable:
             U = ops.radial_table(rel_dist, plan['utab'], plan['D'], plan['ones_col'], stats)
         else:
             U, g = ops.radial_trunk_u(feat, pk['trunk'], plan['Vstack'], plan['gmean'], plan['ones_col'], stats, want_g=not covered)
-        lr = dict(plan['pairs'])
-        check = (conv, stats, plan['have'])
-        if geom is not None and geom.deferred is not None:
-            geom.deferred.append(check)          # checked once per forward by the caller
-        elif check_lowrank_stats([check]):
+        lr = dict(d.lr)
+        if not d.deferred and check_lowrank_stats([(conv, stats, plan['have'])]):
             # the fp32 trunk outputs of this forward leave the cached subspace (distances beyond the plan's range)
             if conv.free_master:
                 raise LowRankPlanMiss('low-rank radial plan does not cover this input; pack_weights(max_distance=...) was given too '
@@ -635,15 +797,22 @@ def conv_dispatch(conv, edge_info, rel_dist, geom, capturing):
     elif len(lr) < len(conv.pairs) and g is None:
         g = ops.radial_trunk(feat, pk['trunk'], len(conv.pairs))       # the direct kernels consume g itself
     how = {pair: lr[pair]['kind'] if pair in lr else 'tc' if tc_ok[pair] else 'simt' for pair in conv.pairs}
-    outs = {do: torch.empty((E, mo, to_order(do)), dtype=torch.float32, device=dev) for do, mo in conv.fiber_out}
+    # (the production route allocates the outputs it writes in _production_forward: pooled ones go to the nodes directly)
+    outs = {} if route == 'production' else \
+        {do: torch.empty((E, mo, to_order(do)), dtype=torch.float32, device=dev) for do, mo in conv.fiber_out}
     return ConvDispatch(conv, sw, route, U, g, lr, plan['z'] if route == 'production' else None, how, outs)
 
 
-def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False):
+def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False, decisions=None, self_out=None, sx=None):
     """Evaluate one or more ConvSE3 that share input features, graph and fibers (to_k / to_v of an attention block)
     in a single sweep: the T blocks (gather x basis) are built once per (degree pair, edge chunk) and consumed by every
     convolution's fused pairwise kernel.  conv_dispatch chooses each convolution's route; the production convolutions run
-    first, then the edge-aligned ones, then the R-first ones (the last two share one T workspace)."""
+    first, then the edge-aligned ones, then the R-first ones (the last two share one T workspace).
+
+    basis: (flat, BasisPlan, Geometry), or (None, None, Geometry) to build the flat basis from the Geometry only if an R-first
+    route needs it.  For one node chunk of a larger graph (NodeChunk), the caller passes the chunk's edges, the features as
+    NodeChunk.src gives them, the chunk's Geometry and the whole graph's decisions (conv_decide), plus the chunk's rows of the
+    whole graph's self-interaction (self_out, one pooled convolution) and edge scales (sx [b', n', k], production route)."""
     c0 = convs[0]
     forward_only_guard('ConvSE3', convs, list(inp.values()) + [rel_dist])
     idx = edge_info[0]
@@ -654,26 +823,30 @@ def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False):
                         "drop-in get_basis() is the reference's per-pair view of the same buffer and is not accepted here")
     flat, plan = basis[:2]                   # BasisFlat (+ Geometry)
     geom = basis[2] if len(basis) > 2 else None
-    bpairs = ops.basis_pairs(flat, plan, E)
     capturing = torch.cuda.is_current_stream_capturing()
     states = []
-    for conv in convs:
+    for conv, decision in zip(convs, decisions or [None] * len(convs)):
         assert conv.pairs == c0.pairs and conv.in_dim == c0.in_dim
-        states.append(conv_dispatch(conv, edge_info, rel_dist, geom, capturing))
+        states.append(conv_dispatch(conv, edge_info, rel_dist, geom, capturing, decision))
+    if self_out is not None:
+        assert len(states) == 1
+        states[0].self_out = self_out
     routes = {r: [st for st in states if st.route == r] for r in ('production', 'aligned', 'rfirst')}
     if routes['production']:
-        _production_forward(routes['production'], inp, edge_info, geom, keep_aligned)
+        _production_forward(routes['production'], inp, edge_info, geom, keep_aligned, sx)
     # the R-first routes chunk over edge tiles so that the largest T block fits the workspace
     t_bytes = max(ops.t_numel(1, mi, to_order(min(di, do)), to_order(do)) * 4 for di, mi in c0.fiber_in for do, _ in c0.fiber_out)
     workspace = None
     if routes['aligned']:
         workspace = _aligned_forward(routes['aligned'], inp, idx, geom, t_bytes, workspace)
     if routes['rfirst']:
-        _rfirst_forward(routes['rfirst'], inp, idx, bpairs, t_bytes, workspace)
+        if flat is None:
+            flat, plan = geom.basis()
+        _rfirst_forward(routes['rfirst'], inp, idx, ops.basis_pairs(flat, plan, E), t_bytes, workspace)
     return [_conv_results(st, inp, edge_info) for st in states]
 
 
-def _production_forward(states, inp, edge_info, geom, keep_aligned):
+def _production_forward(states, inp, edge_info, geom, keep_aligned, sx=None):
     """DESIGN.md 4.5: the neighbour features rotated into the edge frame once per input degree and edge chunk, ONE GEMM per
     (conv, degree_out, |m|) over all input degrees, then the rotation back: fused with the masked mean and the self-interaction
     for pooled convolutions (conv_in / conv_out), or left to the attention kernel with keep_aligned."""
@@ -681,17 +854,26 @@ def _production_forward(states, inp, edge_info, geom, keep_aligned):
     b, n, k = idx.shape
     fiber_in = states[0].conv.fiber_in
     frames = geom.frames()
-    sx = ops.edge_scale(inp, idx, max(di for di, _ in fiber_in))
-    chunks = list(edge_chunks(idx.numel(), sum(mi * to_order(di) for di, mi in fiber_in) * ops.TILE_E * 4))
-    fuse_pool = all(e0 % k == 0 for _, _, e0, _ in chunks)      # the fused pool needs chunks of whole neighbour lists
+    # (a node chunk's view of the features holds the node maxima of its own rows only: it takes the whole graph's scales)
+    assert sx is not None or geom.whole is geom, 'the production route of a node chunk needs the whole graph\'s edge scales'
+    sx = ops.edge_scale(inp, idx, max(di for di, _ in fiber_in)) if sx is None else sx.reshape(-1)
+    tile_bytes = sum(mi * to_order(di) for di, mi in fiber_in) * ops.TILE_E * 4
+    chunks = list(edge_chunks(idx.numel(), tile_bytes))
+    # the fused pool needs edge chunks of whole neighbour lists; decided on the whole graph, so that every node chunk of it
+    # pools the same way (whole-graph chunks of whole lists imply the same for the fewer edges of a node chunk)
+    fuse_pool = all(e0 % k == 0 for _, _, e0, _ in edge_chunks(geom.whole.rel_pos.numel() // 3, tile_bytes))
     for st in states:
         conv = st.conv
         if conv.pool and fuse_pool:
             st.pooled = {do: torch.empty((b * n, mo, to_order(do)), dtype=torch.float32, device=idx.device) for do, mo in conv.fiber_out}
-            st.self_out = conv.self_interact(inp) if conv.self_interaction else {}
+            if st.self_out is None:
+                st.self_out = conv.self_interact(inp) if conv.self_interaction else {}
         elif keep_aligned:                   # the consumer (attention) rotates back on the fly: keep out' itself
             st.aligned_out = {do: torch.empty((idx.numel(), to_order(do), mo), dtype=torch.float32, device=idx.device)
                               for do, mo in conv.fiber_out if do > 0}
+        if st.pooled is None:
+            st.outs = {do: torch.empty((idx.numel(), mo, to_order(do)), dtype=torch.float32, device=idx.device)
+                       for do, mo in conv.fiber_out if do not in st.aligned_out}
     nmask_flat = None if nmask is None else nmask.reshape(-1)
     for t0, tc, e0, ec in chunks:
         X = {di: ops.rotgather(inp[str(di)], idx, frames.D[di] if di > 0 else None, t0, tc) for di, _ in fiber_in}
@@ -834,7 +1016,7 @@ def _conv_results(st, inp, edge_info):
             o = st.outs[do].view(b, n, k, mo, to_order(do))
             outputs[str(do)] = ops.pool(o, nmask) if conv.pool else o
     if conv.self_interaction:
-        outputs = residual_add(outputs, conv.self_interact(inp))
+        outputs = residual_add(outputs, conv.self_interact(inp) if st.self_out is None else st.self_out)
     return outputs
 
 
@@ -912,25 +1094,19 @@ class AttentionSE3(nn.Module):
 
     def forward(self, features, edge_info, rel_dist, basis, global_feats=None, pos_emb=None, mask=None, residual=None):
         forward_only_guard('AttentionSE3', [self], list(features.values()))
-        idx, nmask, _ = edge_info
+        idx = edge_info[0]
         queries = self.to_q(features)
-        k_idx = None
         geom = basis[2] if isinstance(basis, tuple) and len(basis) > 2 else None
         # rotate-back fused into the attention kernel
         fuse = geom is not None and not switches.current().no_attn_rotate and ops.attn_aligned_supported(self.dim_head)
-        if self.linear_proj_keys:
-            values = conv_forward([self.to_v], features, edge_info, rel_dist, basis, keep_aligned=fuse)[0]
-            keys = self.to_k(features)            # node level; the attention kernel gathers through idx
-            k_idx = idx
-        elif self.to_k is None:
-            values = conv_forward([self.to_v], features, edge_info, rel_dist, basis, keep_aligned=fuse)[0]
-            keys = values
-        else:
-            keys, values = conv_forward([self.to_k, self.to_v], features, edge_info, rel_dist, basis, keep_aligned=fuse)
+        # node-level work over the whole graph: node keys (linear_proj_keys), self and global keys / values, rotary queries
+        node_keys = self.to_k(features) if self.linear_proj_keys else None
+        self_keys = self_values = global_keys = global_values = None
         if self.attend_self:
             self_keys, self_values = self.to_self_k(features), self.to_self_v(features)
         if exists(global_feats):
             global_keys, global_values = self.to_global_k(global_feats), self.to_global_v(global_feats)
+        k_emb = None
         if exists(pos_emb):
             # rotary embeddings on the type-0 queries / keys / values (reference S:488-494, 623-629; rotary.py:15-24): cheap
             # elementwise glue in torch around the attention kernel.  The key embedding has 1 + k positions, self first.
@@ -940,28 +1116,75 @@ class AttentionSE3(nn.Module):
             Dh, hk = self.dim_head, (1 if self.one_headed else self.heads)
             queries = dict(queries)
             queries['0'] = apply_rotary_pos_emb(queries['0'].view(b_, n_, self.heads, Dh, 1), q_emb[:, :, None, :, None]).reshape(b_, n_, -1, 1)
+            self_emb = k_emb[:, :, 0, None, :, None]
+            self_keys, self_values = dict(self_keys), dict(self_values)
+            self_keys['0'] = apply_rotary_pos_emb(self_keys['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
+            self_values['0'] = apply_rotary_pos_emb(self_values['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
+        convs = [self.to_v] if self.linear_proj_keys or self.to_k is None else [self.to_k, self.to_v]
+        capturing = torch.cuda.is_current_stream_capturing()
+        decisions = [conv_decide(conv, idx.numel(), rel_dist, geom, capturing) for conv in convs]
+        b, n, k = idx.shape
+        chunks = [NodeChunk(0, b, 0, n, whole=True)]
+        if geom is not None:
+            ckv = self.to_v.fiber_out[0]
+            chunks = geom.node_chunks(decisions, idx.shape, keep_aligned=fuse,
+                                      attn_bytes=0 if k_emb is None else 4 * ckv * (4 + self.linear_proj_keys) + 4 * k_emb.shape[-1])
+        kv = (node_keys, self_keys, self_values, global_keys, global_values)
+        if len(chunks) == 1:
+            outputs = self._attend(chunks[0], features, queries, kv, k_emb, edge_info, rel_dist, basis, geom, decisions, fuse, None)
+        else:
+            sx = chunk_edge_scale(decisions, features, idx)
+            outputs = {d: torch.empty_like(q) for d, q in queries.items()}
+            for c in chunks:
+                cgeom = geom.chunk(c)
+                res = self._attend(c, features, queries, kv, k_emb, edge_info, rel_dist, (None, None, cgeom), cgeom, decisions, fuse,
+                                   c.rows(sx))
+                for d, t in res.items():
+                    c.rows(outputs[d]).copy_(t)
+        if isinstance(self.to_out, LinearSE3):
+            return self.to_out(outputs, residual=residual)             # residual added in the epilogue of to_out
+        return outputs if residual is None else residual_add(outputs, residual)
+
+    def _attend(self, c, features, queries, kv, k_emb, edge_info, rel_dist, basis, geom, decisions, fuse, sx):
+        """The edge work of node chunk c: keys / values of its edges (the convolutions under the whole graph's decisions), then
+        attention of its queries -> {degree: [b', n', H*Dh, 2d+1]}.  geom: the chunk's Geometry (basis[2]); sx: the chunk's rows
+        of the whole graph's edge scales (chunk_edge_scale), None for the whole graph."""
+        node_keys, self_keys, self_values, global_keys, global_values = kv
+        edge_info = c.edge_info(edge_info)
+        idx, nmask, _ = edge_info
+        src = c.src(features)
+        k_idx = None
+        if self.linear_proj_keys:
+            values = conv_forward([self.to_v], src, edge_info, c.rows(rel_dist), basis, keep_aligned=fuse, decisions=decisions, sx=sx)[0]
+            keys = c.src(node_keys)               # node level; the attention kernel gathers through idx
+            k_idx = idx
+        elif self.to_k is None:
+            values = conv_forward([self.to_v], src, edge_info, c.rows(rel_dist), basis, keep_aligned=fuse, decisions=decisions, sx=sx)[0]
+            keys = values
+        else:
+            keys, values = conv_forward([self.to_k, self.to_v], src, edge_info, c.rows(rel_dist), basis, keep_aligned=fuse,
+                                        decisions=decisions, sx=sx)
+        if k_emb is not None:
+            b_, n_, kk = idx.shape
+            Dh, hk = self.dim_head, (1 if self.one_headed else self.heads)
             if k_idx is not None:                                      # linear_proj_keys: keys live on the nodes; rotary is per edge
                 keys = dict(keys)
-                keys['0'] = keys['0'][torch.arange(b_, device=idx.device)[:, None, None], idx]
-            nb_emb, self_emb = k_emb[:, :, 1:, None, :, None], k_emb[:, :, 0, None, :, None]
-            kk = idx.shape[-1]
+                keys['0'] = node_keys['0'][c.b0:c.b1][torch.arange(b_, device=idx.device)[:, None, None], idx]
+            nb_emb = c.rows(k_emb)[:, :, 1:, None, :, None]
             new_k = apply_rotary_pos_emb(keys['0'].view(b_, n_, kk, hk, Dh, 1), nb_emb).reshape(b_, n_, kk, -1, 1)
             new_v = new_k if values is keys else apply_rotary_pos_emb(values['0'].view(b_, n_, kk, hk, Dh, 1), nb_emb).reshape(b_, n_, kk, -1, 1)
             keys, values = dict(keys), dict(values)
             keys['0'], values['0'] = new_k, new_v
-            self_keys, self_values = dict(self_keys), dict(self_values)
-            self_keys['0'] = apply_rotary_pos_emb(self_keys['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
-            self_values['0'] = apply_rotary_pos_emb(self_values['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
         outputs = {}
         for degree in features.keys():
             kw = {}
             if self.attend_self:
-                kw.update(self_k=self_keys[degree], self_v=self_values[degree])
+                kw.update(self_k=c.rows(self_keys[degree]), self_v=c.rows(self_values[degree]))
             if self.use_null_kv:
                 kw.update(null_k=self.null_keys[degree].reshape(-1, to_order(int(degree))),
                           null_v=self.null_values[degree].reshape(-1, to_order(int(degree))))
-            if exists(global_feats) and degree == '0':
-                kw.update(global_k=global_keys[degree], global_v=global_values[degree])
+            if global_keys is not None and degree == '0':
+                kw.update(global_k=global_keys[degree][c.b0:c.b1], global_v=global_values[degree][c.b0:c.b1])
             kd, vd = keys[degree], values[degree]
             if isinstance(vd, AlignedKV) or isinstance(kd, AlignedKV):
                 if isinstance(kd, AlignedKV) and not isinstance(vd, AlignedKV):
@@ -970,12 +1193,10 @@ class AttentionSE3(nn.Module):
                     k_al = isinstance(kd, AlignedKV)
                     kw.update(D=geom.frames().D[int(degree)], k_aligned=k_al)
                     kd, vd = (kd.t if k_al else kd), vd.t
-            outputs[degree] = ops.attention(queries[degree], kd, vd, heads=self.heads, dim_head=self.dim_head,
-                                            scale=self.scale, nmask=nmask, k_idx=(None if exists(pos_emb) and degree == '0' else k_idx),
+            outputs[degree] = ops.attention(c.rows(queries[degree]), kd, vd, heads=self.heads, dim_head=self.dim_head,
+                                            scale=self.scale, nmask=nmask, k_idx=(None if k_emb is not None and degree == '0' else k_idx),
                                             kv_heads=1 if self.one_headed else self.heads, **kw)
-        if isinstance(self.to_out, LinearSE3):
-            return self.to_out(outputs, residual=residual)             # residual added in the epilogue of to_out
-        return outputs if residual is None else residual_add(outputs, residual)
+        return outputs
 
 
 class SinusoidalEmbeddings(nn.Module):
@@ -1502,7 +1723,10 @@ class SE3Transformer(nn.Module):
         Returns (output, the deferred run-time checks of the low-rank plans)."""
         geom = Geometry(rel_pos, self.num_degrees - 1)
         geom.deferred = []
-        basis = ops.basis_flat(rel_pos, self.num_degrees - 1) + (geom,)
+        # every ConvSE3 and attention block runs its edge work over node chunks under this budget (DESIGN.md 4.7); the flat
+        # basis is built by the Geometry of a chunk (or of the whole graph) only when an R-first convolution reads it
+        geom.edge_budget = edge_budget_bytes(switches.current(), rel_pos.device)
+        basis = (None, None, geom)
         x = self.conv_in(feats, edge_info, rel_dist=rel_dist, basis=basis)
         for conv, nonlin in self.convs:
             x = nonlin(x)

@@ -20,6 +20,10 @@ implementations of the same forward (or tunes one); none changes what the model 
 | SE3B200_Z_FLUSH             | z_flush           | unset            | tensor-core accumulator drain period in stages (unset: 8; the     |
 |                             |                   |                  | m > 0 GEMMs of mode 3 also drain at the end of every weight set)  |
 | SE3B200_Z_FLUSH_MULT        | z_flush_mult      | 1                | multiplies the drain period of the ConvSE3 GEMMs                  |
+| SE3B200_EDGE_BUDGET_MB      | edge_budget_mb    | unset            | MiB (2^20 bytes) that the edge-level tensors of one ConvSE3 or    |
+|                             |                   |                  | attention block may take: its edge work runs over node chunks     |
+|                             |                   |                  | sized to fit (model.plan_node_chunks; the result is bit-identical)|
+|                             |                   |                  | unset: a quarter of the device's total memory; 0: one-node chunks |
 
 The model reads `current()` once per ConvSE3 dispatch, LinearSE3 / AttentionSE3 call, Geometry and pack_weights; ConvSE3
 rebuilds its cached dispatch decisions when a switch they depend on changes.  A captured CUDA graph (GraphedForward) replays
@@ -48,6 +52,7 @@ class Switches:
     host_frames: bool = False
     z_flush: int = None
     z_flush_mult: int = 1
+    edge_budget_mb: float = None
 
     def zgemm_flush(self, mode):
         """flush_stages of se3_zgemm_fwd: 0 (the library's default) unless SE3B200_Z_FLUSH or SE3B200_Z_FLUSH_MULT is set."""
