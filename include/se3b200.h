@@ -5,8 +5,8 @@
  * path binds at the three tensor-only seams of the reference (SURVEY.md section 8b):
  *
  *   neighbour builder inside SE3Transformer.forward   se3_transformer_pytorch.py:1171-1294  -> se3_knn_fwd
- *     (packed batches of clouds of different sizes, SE3Transformer.forward_packed: se3_knn_varlen_fwd; no reference counterpart)
- *     (sparse pair inputs: se3_knn_csr_fwd and se3_pair_lookup_fwd; no reference counterpart)
+ *     (also for packed batches of clouds of different sizes, SE3Transformer.forward_packed, and for sparse pair inputs with
+ *      se3_pair_lookup_fwd; no reference counterpart)
  *   get_basis(r_ij, max_degree)                        basis.py:153-205                      -> se3_basis_fwd
  *   RadialFunc trunk (net.0 .. net.5)                  se3_transformer_pytorch.py:287-293    -> se3_radial_trunk_fwd
  *   PairwiseConv + ConvSE3 inner product               se3_transformer_pytorch.py:237-254,
@@ -45,47 +45,43 @@ extern "C" {
 #define SE3_TILE_IF        4  /* (in-channel, frequency) pairs per tile step */
 
 const char* se3_last_error(void);
-int         se3_abi_version(void);     /* 2; raised with every incompatible change of the entry points below */
+int         se3_abi_version(void);     /* 3; raised with every incompatible change of the entry points below */
 
-/* Neighbour graph (S:1171-1294).  For every node i of every cloud: the k smallest "modified" distances over the
- * other n-1 nodes, ascending (ties: lower node index first), exactly as the reference's remove-self + topk:
+/* One pair mask of se3_knn_fwd, dense or as sorted column lists.  shared != 0: one matrix / list for every cloud.
+ *   dense: uint8, pair (i, j) of cloud c at base_c + i n_c + j; base_c = 0 if shared, else c n^2 (uniform) or pair_off[c] (packed).
+ *   cols != NULL: row r is cols[row_ptr[r] .. row_ptr[r+1]) (int64 row pointers, int32 columns [nnz], ascending and unique per
+ *     row; a diagonal entry is ignored; no length limit) with r = i if shared, else the node index c n + i.  Row pointers are
+ *     clamped to [0, nnz]. */
+typedef struct se3_pairs {
+  const uint8_t* dense;
+  const int64_t* row_ptr;
+  const int* cols;
+  int64_t nnz;
+  int shared;
+} se3_pairs;
+
+/* Neighbour graph (S:1171-1294).  For every node i of every cloud: the k smallest "modified" distances over the other nodes of
+ * its cloud, ascending (ties: lower node index first), exactly as the reference's remove-self + topk:
  *   modified = true distance; user neighbor_mask==0 -> FLT_MAX (S:1257); bonded (sparse_adj!=0) -> 0 (S:1262);
  *   causal and j' >= i on the self-removed grid -> FLT_MAX (S:1266-1268).
- * out_mask = (modified <= valid_radius) & node_mask[i] & node_mask[j]  (S:1284, 1290-1291).
- * node_mask, neighbor_mask, sparse_adj may be NULL.  Requires 1 <= b <= 65535 and 1 <= k <= min(n-1, 4096); n is bounded by
- * the grid only (one CTA per node).  A row of up to 4096 columns is sorted whole in shared memory; a longer row is searched in
- * tiles of 4096 columns merged into a running list of the best next_pow2(k) keys, with the same keys, tie rule and results. */
-int se3_knn_fwd(const float* coors, const uint8_t* node_mask, const uint8_t* neighbor_mask, const uint8_t* sparse_adj,
-                int b, int n, int k, float valid_radius, int causal,
-                int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream);
+ * out_mask = (modified <= valid_radius) & node_mask[i] & node_mask[j]  (S:1284, 1290-1291).  Both pair forms give the same bits.
+ * A row of up to 4096 columns is sorted whole in shared memory; a longer one in tiles of 4096 columns merged into a running list
+ * of the best next_pow2(k) keys, with the same results.  One CTA per node: < 2^31 nodes (the batch size has no limit of its own).
+ * Outputs out_idx / out_mask / out_rel_dist [nodes, K], out_rel_pos [nodes, K, 3]; node_mask [nodes] and both masks may be NULL.
+ *   uniform (cu_seqlens == NULL): b clouds of n nodes, coors [b, n, 3], K = k with 1 <= k <= min(n-1, 4096), indices local to
+ *     the cloud.  Reads nothing back, so a CUDA graph can capture it.
+ *   packed: b clouds of n_c = cu_seqlens[c+1] - cu_seqlens[c] nodes end to end, coors [n, 3] (n = all nodes), each searched as the
+ *     uniform form with b = 1, n = n_c, k = k_per_cloud[c]; its first k_c slots are bit-identical to that, slots past them
+ *     repeat slot k_c - 1 with mask 0, and indices are global (cu_seqlens[c] added).  K = k.  cu_seqlens [b+1] int64,
+ *     k_per_cloud [b] int32 and pair_off [b] int64 (with dense masks) are DEVICE arrays; the call reads them back (one
+ *     synchronisation of `stream`) and refuses n_c outside [2, 4097], k_c outside [1, n_c - 1], K < k_c and bad offsets.
+ * Refused (SE3_EINVAL): a dense mask with a column list; with packed clouds a node mask, column lists or a shared mask. */
+int se3_knn_fwd(const float* coors, const int64_t* cu_seqlens, const int* k_per_cloud, const int64_t* pair_off,
+                const uint8_t* node_mask, const se3_pairs* neighbor_mask, const se3_pairs* sparse_adj, int b, int64_t n, int k,
+                float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist,
+                void* stream);
 
-/* Neighbour graph of a packed batch: clouds c = 0 .. num_clouds-1 of n_c = cu_seqlens[c+1] - cu_seqlens[c] nodes laid end to end,
- * coors [total, 3].  Each cloud is searched on its own, exactly as se3_knn_fwd(b = 1, n = n_c, k = k_per_cloud[c]) with no node
- * mask (same keys, tie rule, arithmetic and mask rule: the first k_c slots of a row are bit-identical to it), and the indices are
- * global (start_c added).  Outputs have K >= max k_c slots per node: out_idx / out_mask / out_rel_dist [total, K],
- * out_rel_pos [total, K, 3]; slots r >= k_c repeat slot k_c - 1 with mask 0.  neighbor_mask / sparse_adj: the clouds' [n_c, n_c]
- * matrices flattened end to end ([sum n_c^2] uint8), pair (i, j) of cloud c at pair_off[c] + i n_c + j; either may be NULL
- * (pair_off may be NULL when both are).  cu_seqlens [num_clouds+1] int64, k_per_cloud [num_clouds] int32, pair_off [num_clouds]
- * int64 are DEVICE arrays; the call reads them back (one synchronisation of `stream`) and refuses n_c outside [2, 4097] or
- * above max_len, k_c outside [1, n_c - 1], K < k_c and inconsistent offsets. */
-int se3_knn_varlen_fwd(const float* coors, const int64_t* cu_seqlens, const int* k_per_cloud, const uint8_t* neighbor_mask,
-                       const uint8_t* sparse_adj, const int64_t* pair_off, int num_clouds, int64_t total, int K, int max_len,
-                       float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos,
-                       float* out_rel_dist, void* stream);
-
-/* se3_knn_fwd with the pair masks given as sparse rows instead of [b, n, n] bytes (SE3Transformer.forward with torch.sparse_coo
- * pair inputs).  A list is int64 row pointers ptr and int32 columns cols [nnz]: row (b, i) is cols[ptr[r] .. ptr[r+1]) with
- * r = b * batch_stride + i, columns ascending and unique per row (a diagonal entry is allowed and ignored).  batch_stride is n
- * (ptr has b*n + 1 entries) or 0 (ptr has n + 1 entries: one list shared by the batch).  A column listed in row (b, i) of the
- * neighbour list is allowed and one missing from it gets distance FLT_MAX; a column of the bonded list gets distance 0; causal
- * overrides both -- the precedence, keys, tie rule and results of se3_knn_fwd on the densified masks, bit for bit.  Either list
- * may be NULL (cols == NULL); rows have no length limit.  Row pointers are clamped to [0, nnz]. */
-int se3_knn_csr_fwd(const float* coors, const uint8_t* node_mask, const int64_t* nbr_ptr, const int* nbr_cols, int64_t nbr_nnz,
-                    int64_t nbr_batch_stride, const int64_t* adj_ptr, const int* adj_cols, int64_t adj_nnz,
-                    int64_t adj_batch_stride, int b, int n, int k, float valid_radius, int causal, int64_t* out_idx,
-                    uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream);
-
-/* Position of every neighbour in a sparse pair list (row pointers and columns as in se3_knn_csr_fwd): out[b,i,kk] = p with
+/* Position of every neighbour in a sparse pair list (as in se3_pairs; batch_stride 0 when shared, else n): out[b,i,kk] = p with
  * cols[p] == idx[b,i,kk] inside row (b, i), or -1 if the row lacks that column.  idx, out: [b, n, k] int64.  The caller indexes
  * the list's values (edge tokens, edge features, hop counts) with a zero row appended for -1. */
 int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx, int b, int n,

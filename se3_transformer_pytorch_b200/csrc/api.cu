@@ -12,4 +12,4 @@ void set_error(const char* fmt, ...) {
 }  // namespace se3
 
 extern "C" const char* se3_last_error(void) { return se3::g_err; }
-extern "C" int se3_abi_version(void) { return 2; }
+extern "C" int se3_abi_version(void) { return 3; }

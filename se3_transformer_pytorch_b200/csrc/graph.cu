@@ -3,11 +3,13 @@
 // Replaces the dense [b,n,n-1] temporaries + torch.topk + batched_index_select of the reference
 // (se3_transformer_pytorch.py:1171-1294, utils.py:56-80) with one CTA per query node that sorts (distance, column) keys of its
 // row bitonically in shared memory and emits only the k winners.  A row of up to KNN_TILE columns is sorted whole; a longer one
-// is walked in tiles of KNN_TILE columns, each merged into a running list of the best next_pow2(k) keys.  The same row body
-// serves padded batches [b, n] (knn_kernel), packed batches of clouds of different sizes (knn_varlen_kernel) and pair masks
-// given as sorted column lists (knn_csr_kernel; pair_lookup_kernel finds a neighbour's pair in such a list).
+// is walked in tiles of KNN_TILE columns, each merged into a running list of the best next_pow2(k) keys.  One kernel,
+// knn_kernel, serves padded batches [b, n] and packed batches of clouds of different sizes, with pair masks given as bytes
+// (DensePairs) or as sorted column lists (CsrPairs; pair_lookup_kernel finds a neighbour's pair in such a list).
 #include "common.cuh"
 #include <cfloat>
+#include <algorithm>
+#include <type_traits>
 #include <vector>
 
 namespace se3 {
@@ -125,8 +127,8 @@ __device__ __forceinline__ void knn_sort(unsigned long long* keys, int npad) {
   }
 }
 
-// The neighbour list of node i of one cloud of n nodes (c = that cloud's coordinates, [n, 3]); shared by the padded
-// (knn_kernel), the packed (knn_varlen_kernel) and the CSR (knn_csr_kernel) search so that all produce the same bits.  pairs:
+// The neighbour list of node i of one cloud of n nodes (c = that cloud's coordinates, [n, 3]); the same body for every cloud
+// form and pair form of knn_kernel, so that all produce the same bits.  pairs:
 // row i of the cloud's pair masks (DensePairs or CsrPairs); node_mask: the cloud's [n] node mask (or NULL).  Writes slots
 // [0, K_out) of the row at out_*; slots r >= k are copies of slot k - 1 with mask 0, and indices are offset by j_base.
 // keys: npad = next_pow2(n - 1) keys of shared memory when n - 1 <= KNN_TILE (one sort of the whole row), otherwise
@@ -188,78 +190,60 @@ __device__ __forceinline__ void knn_row(unsigned long long* keys, const float* _
   }
 }
 
-// One CTA per (cloud, node i) of a padded batch [b, n].  Both kernels ask for 6 CTAs per SM: without it the tiled branch of
-// knn_row raises them from 40 to 48 registers, and whole-row searches would lose a CTA per SM.
-template <int THREADS>
+// Row pointers of row r of a column list, clamped to [0, nnz] so that a malformed list reads no memory outside it.
+__device__ __forceinline__ void csr_bounds(const se3_pairs& p, int64_t r, int64_t& lo, int64_t& hi) {
+  lo = min(max(p.row_ptr[r], (int64_t)0), p.nnz);
+  hi = min(max(p.row_ptr[r + 1], lo), p.nnz);
+}
+
+// One CTA per node t of the flat node list.  Uniform clouds (cu_seqlens NULL): cloud c = t / n of n nodes, K = k, indices
+// local to the cloud.  Packed clouds: the CTA finds its cloud by binary search in cu_seqlens, searches it for k_per_cloud[c]
+// neighbours and writes K >= k_c slots with global indices; dense pair masks are the clouds' [n_c, n_c] matrices flattened
+// end to end, cloud c starting at pair_off[c].  A shared pair input (one matrix or list for every cloud) is read at row i.
+// Shared memory: key_words keys (see knn_row), then the two bitmaps of CsrPairs.  Both instantiations ask for 6 CTAs per SM:
+// without it the tiled branch of knn_row raises them from 40 to 48 registers, and whole-row searches would lose a CTA per SM.
+template <int THREADS, class Pairs>
 __global__ void __launch_bounds__(THREADS, 6)
-knn_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mask,
-           const uint8_t* __restrict__ neighbor_mask, const uint8_t* __restrict__ sparse_adj,
-           int n, int k, int npad, float valid_radius, int causal,
+knn_kernel(const float* __restrict__ coors, const int64_t* __restrict__ cu_seqlens, const int* __restrict__ k_per_cloud,
+           const int64_t* __restrict__ pair_off, const uint8_t* __restrict__ node_mask, const se3_pairs nbr, const se3_pairs adj,
+           int num_clouds, int n, int K, int key_words, float valid_radius, int causal,
            int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
            float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
   extern __shared__ unsigned long long keys[];
-  const int i = blockIdx.x, b = blockIdx.y;
-  const size_t row = ((size_t)b * n + i) * n;
-  const size_t o = ((size_t)b * n + i) * k;
-  knn_row<THREADS>(keys, coors + (size_t)b * n * 3, n, i, k, npad,
-                   DensePairs{neighbor_mask ? neighbor_mask + row : nullptr, sparse_adj ? sparse_adj + row : nullptr},
-                   node_mask ? node_mask + (size_t)b * n : nullptr, valid_radius, causal, k, 0, out_idx + o, out_mask + o,
-                   out_rel_pos + o * 3, out_rel_dist + o);
-}
-
-// knn_kernel with the pair masks given as CSR rows: row (b, i) of a list is entries [ptr[r], ptr[r+1]) of its columns, with
-// r = b * batch_stride + i (batch_stride 0: one [n, n] list shared by the batch).  Row pointers are clamped to [0, nnz], so a
-// malformed list reads no memory outside it.  Shared memory: the keys of knn_kernel, then the two bitmaps of CsrPairs.
-template <int THREADS>
-__global__ void __launch_bounds__(THREADS, 6)
-knn_csr_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mask,
-               const int64_t* __restrict__ nbr_ptr, const int* __restrict__ nbr_cols, int64_t nbr_nnz, int64_t nbr_stride,
-               const int64_t* __restrict__ adj_ptr, const int* __restrict__ adj_cols, int64_t adj_nnz, int64_t adj_stride,
-               int n, int k, int npad, int key_words, float valid_radius, int causal,
-               int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
-               float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
-  extern __shared__ unsigned long long keys[];
-  const int i = blockIdx.x, b = blockIdx.y;
-  const size_t o = ((size_t)b * n + i) * k;
-  CsrPairs pairs{nbr_cols, adj_cols, 0, 0, 0, 0, reinterpret_cast<unsigned*>(keys + key_words), 0};
-  if (nbr_cols) {
-    const int64_t r = (int64_t)b * nbr_stride + i;
-    pairs.nbr_lo = min(max(nbr_ptr[r], (int64_t)0), nbr_nnz);
-    pairs.nbr_hi = min(max(nbr_ptr[r + 1], pairs.nbr_lo), nbr_nnz);
-  }
-  if (adj_cols) {
-    const int64_t r = (int64_t)b * adj_stride + i;
-    pairs.adj_lo = min(max(adj_ptr[r], (int64_t)0), adj_nnz);
-    pairs.adj_hi = min(max(adj_ptr[r + 1], pairs.adj_lo), adj_nnz);
-  }
-  knn_row<THREADS>(keys, coors + (size_t)b * n * 3, n, i, k, npad, pairs, node_mask ? node_mask + (size_t)b * n : nullptr,
-                   valid_radius, causal, k, 0, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
-}
-
-// One CTA per node of a packed batch: clouds c of n_c = cu_seqlens[c+1] - cu_seqlens[c] nodes laid end to end.  The CTA finds
-// its cloud by binary search, searches that cloud only (local columns, the cloud's own k_c) and writes K >= k_c slots with
-// global indices.  Pair masks are the clouds' [n_c, n_c] matrices flattened end to end, cloud c starting at pair_off[c].
-template <int THREADS>
-__global__ void __launch_bounds__(THREADS, 6)
-knn_varlen_kernel(const float* __restrict__ coors, const int64_t* __restrict__ cu_seqlens, const int* __restrict__ k_per_cloud,
-                  const uint8_t* __restrict__ neighbor_mask, const uint8_t* __restrict__ sparse_adj,
-                  const int64_t* __restrict__ pair_off, int num_clouds, int K, float valid_radius, int causal,
-                  int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
-                  float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
-  extern __shared__ unsigned long long keys[];
   const int64_t t = blockIdx.x;
-  int lo = 0, hi = num_clouds - 1;               // the last cloud c with cu_seqlens[c] <= t
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (cu_seqlens[mid] <= t) lo = mid; else hi = mid - 1;
+  int64_t start, base;                              // first node of the cloud, start of its dense pair matrix
+  int n_c, k_c;
+  if (cu_seqlens) {
+    int lo = 0, hi = num_clouds - 1;                // the last cloud c with cu_seqlens[c] <= t
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (cu_seqlens[mid] <= t) lo = mid; else hi = mid - 1;
+    }
+    start = cu_seqlens[lo];
+    n_c = (int)(cu_seqlens[lo + 1] - start);
+    k_c = k_per_cloud[lo];
+    base = pair_off ? pair_off[lo] : 0;
+  } else {
+    start = t / n * n;
+    n_c = n;
+    k_c = K;
+    base = start * n;
   }
-  const int64_t start = cu_seqlens[lo];
-  const int n = (int)(cu_seqlens[lo + 1] - start), i = (int)(t - start);
-  const size_t row = neighbor_mask || sparse_adj ? (size_t)pair_off[lo] + (size_t)i * n : 0;
-  const size_t o = (size_t)t * K;
-  knn_row<THREADS>(keys, coors + start * 3, n, i, k_per_cloud[lo], knn_npad(n),
-                   DensePairs{neighbor_mask ? neighbor_mask + row : nullptr, sparse_adj ? sparse_adj + row : nullptr}, nullptr,
-                   valid_radius, causal, K, start, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
+  const int i = (int)(t - start);
+  Pairs pairs;
+  if constexpr (std::is_same<Pairs, DensePairs>::value) {
+    const int64_t row = (int64_t)i * n_c;
+    pairs = DensePairs{nbr.dense ? nbr.dense + (nbr.shared ? 0 : base) + row : nullptr,
+                       adj.dense ? adj.dense + (adj.shared ? 0 : base) + row : nullptr};
+  } else {
+    pairs = CsrPairs{nbr.cols, adj.cols, 0, 0, 0, 0, reinterpret_cast<unsigned*>(keys + key_words), 0};
+    if (nbr.cols) csr_bounds(nbr, nbr.shared ? i : t, pairs.nbr_lo, pairs.nbr_hi);
+    if (adj.cols) csr_bounds(adj, adj.shared ? i : t, pairs.adj_lo, pairs.adj_hi);
+  }
+  const int64_t o = t * K;
+  knn_row<THREADS>(keys, coors + start * 3, n_c, i, k_c, knn_npad(n_c), pairs, node_mask ? node_mask + start : nullptr,
+                   valid_radius, causal, K, cu_seqlens ? start : 0, out_idx + o, out_mask + o, out_rel_pos + o * 3,
+                   out_rel_dist + o);
 }
 
 __global__ void gather_pairs_kernel(const float* __restrict__ pf, const int64_t* __restrict__ idx, int n, int k, int e,
@@ -273,7 +257,7 @@ __global__ void gather_pairs_kernel(const float* __restrict__ pf, const int64_t*
   out[t] = pf[(bi * n + j) * e + c];
 }
 
-// out[s] = position of column idx[s] in CSR row s / k (clamped to [0, nnz] as in knn_csr_kernel), or -1 if the row lacks it.
+// out[s] = position of column idx[s] in CSR row s / k (clamped to [0, nnz] as in csr_bounds), or -1 if the row lacks it.
 __global__ void pair_lookup_kernel(const int64_t* __restrict__ ptr, const int* __restrict__ cols, int64_t nnz, int64_t stride,
                                    const int64_t* __restrict__ idx, int n, int k, int64_t total, int64_t* __restrict__ out) {
   const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -311,98 +295,66 @@ __global__ void pool_kernel(const float* __restrict__ x, const uint8_t* __restri
 
 }  // namespace se3
 
-extern "C" int se3_knn_fwd(const float* coors, const uint8_t* node_mask, const uint8_t* neighbor_mask,
-                           const uint8_t* sparse_adj, int b, int n, int k, float valid_radius, int causal,
-                           int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream) {
+extern "C" int se3_knn_fwd(const float* coors, const int64_t* cu_seqlens, const int* k_per_cloud, const int64_t* pair_off,
+                           const uint8_t* node_mask, const se3_pairs* neighbor_mask, const se3_pairs* sparse_adj, int b, int64_t n,
+                           int k, float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos,
+                           float* out_rel_dist, void* stream) {
   using namespace se3;
-  SE3_REQUIRE(b > 0 && n > 1, "se3_knn_fwd: need b > 0 and n > 1 (got b=%d n=%d)", b, n);
-  SE3_REQUIRE(k >= 1 && k <= n - 1, "se3_knn_fwd: k must be in [1, n-1] (got k=%d n=%d)", k, n);
-  SE3_REQUIRE(b <= 65535, "se3_knn_fwd: b = %d exceeds the grid's y dimension (65535)", b);
-  SE3_REQUIRE(k <= KNN_TILE, "se3_knn_fwd: k = %d neighbours exceeds %d, the longest list the tiled search keeps in shared memory",
-              k, KNN_TILE);
-  constexpr int THREADS = 256;
-  const bool tiled = n - 1 > KNN_TILE;
-  const int npad = tiled ? KNN_TILE : knn_npad(n);
-  const size_t smem = (size_t)(npad + (tiled ? next_pow2(k) : 0)) * sizeof(unsigned long long);
-  if (smem > 48 * 1024)
-    SE3_CUDA_OK(cudaFuncSetAttribute(knn_kernel<THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  dim3 grid(n, b);
-  knn_kernel<THREADS><<<grid, THREADS, smem, as_stream(stream)>>>(coors, node_mask, neighbor_mask, sparse_adj, n, k, npad,
-                                                                  valid_radius, causal, out_idx, out_mask, out_rel_pos,
-                                                                  out_rel_dist);
-  SE3_LAUNCH_OK();
-  return SE3_OK;
-}
-
-extern "C" int se3_knn_varlen_fwd(const float* coors, const int64_t* cu_seqlens, const int* k_per_cloud,
-                                  const uint8_t* neighbor_mask, const uint8_t* sparse_adj, const int64_t* pair_off, int num_clouds,
-                                  int64_t total, int K, int max_len, float valid_radius, int causal, int64_t* out_idx,
-                                  uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream) {
-  using namespace se3;
-  SE3_REQUIRE(num_clouds > 0 && total > 0 && K > 0, "se3_knn_varlen_fwd: need num_clouds, total, K > 0 (got %d, %lld, %d)",
-              num_clouds, (long long)total, K);
-  SE3_REQUIRE(total < (1ll << 31), "se3_knn_varlen_fwd: %lld nodes exceed the 1-D grid", (long long)total);
-  SE3_REQUIRE(max_len >= 2 && max_len - 1 <= 4096, "se3_knn_varlen_fwd: max_len = %d must be in [2, 4097]", max_len);
-  // the sizes live on the device: read them back once (a few hundred bytes) so that a bad batch is refused, not read out of bounds
-  std::vector<int64_t> cu(num_clouds + 1), off(num_clouds);
-  std::vector<int> kc(num_clouds);
+  const se3_pairs none{nullptr, nullptr, nullptr, 0, 0};
+  const se3_pairs& nbr = neighbor_mask ? *neighbor_mask : none;
+  const se3_pairs& adj = sparse_adj ? *sparse_adj : none;
+  const bool dense = nbr.dense || adj.dense, csr = nbr.cols || adj.cols;
+  SE3_REQUIRE(!(dense && csr), "se3_knn_fwd: the pair masks must both be dense or both be column lists");
+  for (const se3_pairs* p : {&nbr, &adj})
+    SE3_REQUIRE(!p->cols || (p->row_ptr && p->nnz >= 0), "se3_knn_fwd: a column list needs row pointers and nnz >= 0");
+  const int64_t nodes = cu_seqlens ? n : (int64_t)b * n;
+  SE3_REQUIRE(nodes < (1ll << 31), "se3_knn_fwd: %lld nodes exceed the 1-D grid", (long long)nodes);
   cudaStream_t s = as_stream(stream);
-  SE3_CUDA_OK(cudaMemcpyAsync(cu.data(), cu_seqlens, cu.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-  SE3_CUDA_OK(cudaMemcpyAsync(kc.data(), k_per_cloud, kc.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  const bool pairs = neighbor_mask || sparse_adj;
-  if (pairs) SE3_CUDA_OK(cudaMemcpyAsync(off.data(), pair_off, off.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-  SE3_CUDA_OK(cudaStreamSynchronize(s));
-  SE3_REQUIRE(cu[0] == 0 && cu[num_clouds] == total, "se3_knn_varlen_fwd: cu_seqlens must run from 0 to total = %lld (got %lld .. %lld)",
-              (long long)total, (long long)cu[0], (long long)cu[num_clouds]);
-  int64_t pairs_before = 0;
-  for (int c = 0; c < num_clouds; ++c) {
-    const int64_t n = cu[c + 1] - cu[c];
-    SE3_REQUIRE(n >= 2 && n - 1 <= 4096, "se3_knn_varlen_fwd: cloud %d has %lld nodes; each cloud needs 2 .. 4097", c, (long long)n);
-    SE3_REQUIRE(n <= max_len, "se3_knn_varlen_fwd: cloud %d has %lld nodes > max_len = %d", c, (long long)n, max_len);
-    SE3_REQUIRE(kc[c] >= 1 && kc[c] <= n - 1, "se3_knn_varlen_fwd: k of cloud %d must be in [1, n_c - 1] (got k=%d n_c=%lld)", c,
-                kc[c], (long long)n);
-    SE3_REQUIRE(kc[c] <= K, "se3_knn_varlen_fwd: K = %d is smaller than k = %d of cloud %d", K, kc[c], c);
-    SE3_REQUIRE(!pairs || off[c] == pairs_before, "se3_knn_varlen_fwd: pair_off[%d] = %lld, expected sum of n_c^2 before it = %lld", c,
-                (long long)off[c], (long long)pairs_before);
-    pairs_before += n * n;
+  int n_max = (int)n;                               // nodes of the largest cloud
+  if (!cu_seqlens) {
+    SE3_REQUIRE(b > 0 && n > 1, "se3_knn_fwd: need b > 0 and n > 1 (got b=%d n=%lld)", b, (long long)n);
+    SE3_REQUIRE(k >= 1 && k <= n - 1, "se3_knn_fwd: k must be in [1, n-1] (got k=%d n=%lld)", k, (long long)n);
+    SE3_REQUIRE(k <= KNN_TILE, "se3_knn_fwd: k = %d neighbours exceeds %d, the longest list the tiled search keeps in shared memory",
+                k, KNN_TILE);
+  } else {
+    SE3_REQUIRE(!csr && !node_mask && !nbr.shared && !adj.shared,
+                "se3_knn_fwd: packed clouds take neither column lists, a node mask nor a shared pair mask");
+    SE3_REQUIRE(b > 0 && n > 0 && k > 0, "se3_knn_fwd: need num_clouds, total, K > 0 (got %d, %lld, %d)", b, (long long)n, k);
+    SE3_REQUIRE(!dense || pair_off, "se3_knn_fwd: dense pair masks of packed clouds need pair_off");
+    // the sizes live on the device: read them back once (a few hundred bytes) so that a bad batch is refused, not read out of bounds
+    std::vector<int64_t> cu(b + 1), off(b);
+    std::vector<int> kc(b);
+    SE3_CUDA_OK(cudaMemcpyAsync(cu.data(), cu_seqlens, cu.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    SE3_CUDA_OK(cudaMemcpyAsync(kc.data(), k_per_cloud, kc.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (dense) SE3_CUDA_OK(cudaMemcpyAsync(off.data(), pair_off, off.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    SE3_CUDA_OK(cudaStreamSynchronize(s));
+    SE3_REQUIRE(cu[0] == 0 && cu[b] == n, "se3_knn_fwd: cu_seqlens must run from 0 to total = %lld (got %lld .. %lld)",
+                (long long)n, (long long)cu[0], (long long)cu[b]);
+    int64_t pairs_before = 0;
+    n_max = 0;
+    for (int c = 0; c < b; ++c) {
+      const int64_t n_c = cu[c + 1] - cu[c];
+      SE3_REQUIRE(n_c >= 2 && n_c - 1 <= KNN_TILE, "se3_knn_fwd: cloud %d has %lld nodes; each cloud needs 2 .. 4097", c, (long long)n_c);
+      SE3_REQUIRE(kc[c] >= 1 && kc[c] <= n_c - 1, "se3_knn_fwd: k of cloud %d must be in [1, n_c - 1] (got k=%d n_c=%lld)", c,
+                  kc[c], (long long)n_c);
+      SE3_REQUIRE(kc[c] <= k, "se3_knn_fwd: K = %d is smaller than k = %d of cloud %d", k, kc[c], c);
+      SE3_REQUIRE(!dense || off[c] == pairs_before, "se3_knn_fwd: pair_off[%d] = %lld, expected sum of n_c^2 before it = %lld", c,
+                  (long long)off[c], (long long)pairs_before);
+      pairs_before += n_c * n_c;
+      n_max = std::max(n_max, (int)n_c);
+    }
   }
   constexpr int THREADS = 256;
-  const size_t smem = (size_t)knn_npad(max_len) * sizeof(unsigned long long);
-  knn_varlen_kernel<THREADS><<<(unsigned)total, THREADS, smem, s>>>(coors, cu_seqlens, k_per_cloud, neighbor_mask, sparse_adj,
-                                                                     pair_off, num_clouds, K, valid_radius, causal, out_idx,
-                                                                     out_mask, out_rel_pos, out_rel_dist);
-  SE3_LAUNCH_OK();
-  return SE3_OK;
-}
-
-extern "C" int se3_knn_csr_fwd(const float* coors, const uint8_t* node_mask, const int64_t* nbr_ptr, const int* nbr_cols,
-                               int64_t nbr_nnz, int64_t nbr_batch_stride, const int64_t* adj_ptr, const int* adj_cols,
-                               int64_t adj_nnz, int64_t adj_batch_stride, int b, int n, int k, float valid_radius, int causal,
-                               int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream) {
-  using namespace se3;
-  SE3_REQUIRE(b > 0 && n > 1, "se3_knn_csr_fwd: need b > 0 and n > 1 (got b=%d n=%d)", b, n);
-  SE3_REQUIRE(k >= 1 && k <= n - 1, "se3_knn_csr_fwd: k must be in [1, n-1] (got k=%d n=%d)", k, n);
-  SE3_REQUIRE(b <= 65535, "se3_knn_csr_fwd: b = %d exceeds the grid's y dimension (65535)", b);
-  SE3_REQUIRE(k <= KNN_TILE, "se3_knn_csr_fwd: k = %d neighbours exceeds %d, the longest list the tiled search keeps in shared memory",
-              k, KNN_TILE);
-  SE3_REQUIRE(!nbr_cols || (nbr_ptr && nbr_nnz >= 0 && (nbr_batch_stride == 0 || nbr_batch_stride == n)),
-              "se3_knn_csr_fwd: neighbour-mask rows need row pointers, nnz >= 0 and a batch stride of 0 or n");
-  SE3_REQUIRE(!adj_cols || (adj_ptr && adj_nnz >= 0 && (adj_batch_stride == 0 || adj_batch_stride == n)),
-              "se3_knn_csr_fwd: bonded rows need row pointers, nnz >= 0 and a batch stride of 0 or n");
-  constexpr int THREADS = 256;
-  const bool tiled = n - 1 > KNN_TILE;
-  const int npad = tiled ? KNN_TILE : knn_npad(n);
-  const int key_words = npad + (tiled ? next_pow2(k) : 0);
-  const size_t smem = (size_t)key_words * sizeof(unsigned long long) + 2 * CSR_BITMAP_WORDS * sizeof(unsigned);
-  if (smem > 48 * 1024)
-    SE3_CUDA_OK(cudaFuncSetAttribute(knn_csr_kernel<THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  dim3 grid(n, b);
-  knn_csr_kernel<THREADS><<<grid, THREADS, smem, as_stream(stream)>>>(coors, node_mask, nbr_ptr, nbr_cols, nbr_nnz,
-                                                                      nbr_batch_stride, adj_ptr, adj_cols, adj_nnz,
-                                                                      adj_batch_stride, n, k, npad, key_words, valid_radius,
-                                                                      causal, out_idx, out_mask, out_rel_pos, out_rel_dist);
-  SE3_LAUNCH_OK();
-  return SE3_OK;
+  const int key_words = n_max - 1 > KNN_TILE ? KNN_TILE + next_pow2(k) : knn_npad(n_max);
+  const size_t smem = (size_t)key_words * sizeof(unsigned long long) + (csr ? 2 * CSR_BITMAP_WORDS * sizeof(unsigned) : 0);
+  auto launch = [&](auto kernel) -> int {
+    if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<(unsigned)nodes, THREADS, smem, s>>>(coors, cu_seqlens, k_per_cloud, pair_off, node_mask, nbr, adj, b, (int)n, k,
+                                                  key_words, valid_radius, causal, out_idx, out_mask, out_rel_pos, out_rel_dist);
+    SE3_LAUNCH_OK();
+    return SE3_OK;
+  };
+  return csr ? launch(knn_kernel<THREADS, CsrPairs>) : launch(knn_kernel<THREADS, DensePairs>);
 }
 
 extern "C" int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx,

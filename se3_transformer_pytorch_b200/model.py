@@ -1449,36 +1449,12 @@ class SE3Transformer(nn.Module):
         b, n = feats['0'].shape[:2]
         device = feats['0'].device
         feats = self._check_features(feats, coors)
-        neighbors, valid_radius = self.num_neighbors, self.valid_radius
-        assert self.attend_sparse_neighbors or neighbors > 0, 'you must either attend to sparsely bonded neighbors, or set number of locally attended neighbors to be greater than 0'
-
-        if neighbors == 0:
-            valid_radius = 0
-        if any(_is_sparse(t) for t in (adj_mat, edges, neighbor_mask)):
-            idx, nmask, rel_pos, rel_dist, e = self._sparse_graph(coors, mask, adj_mat, edges, neighbor_mask, b, n, valid_radius)
-        else:
-            adj_indices, sparse_mask, num_sparse = self._bonded(adj_mat, b, n, device)
-            total = self._num_neighbors(n, num_sparse)
-            if exists(neighbor_mask):
-                eye = torch.eye(n, dtype=torch.bool, device=neighbor_mask.device)
-                self._report_neighbor_mask(neighbor_mask.masked_fill(eye.unsqueeze(0), False).sum(dim=-1))
-
-            idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=neighbor_mask,
-                                                    sparse_adj=sparse_mask, causal=self.causal)
-
-            # edge features on the neighbour list (reference S:1231-1239, 1293-1294); gather first, embed after
-            e = None
-            if exists(edges):
-                if exists(self.edge_emb):
-                    if edges.dim() == 2:                        # [b, n] tokens: the reference broadcasts them over rows (b == 1)
-                        assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
-                        edges = edges.unsqueeze(1).expand(b, n, n)
-                    e = self.edge_emb(edges.gather(2, idx))
-                else:
-                    e = ops.gather_pairs(edges.float(), idx)
-            if exists(self.adj_emb):
-                a = self.adj_emb(adj_indices.gather(2, idx))
-                e = torch.cat((e, a), dim=-1) if exists(e) else a
+        valid_radius = self._valid_radius()
+        if exists(edges) and exists(self.edge_emb) and edges.dim() == 2:   # [b, n] tokens: the reference broadcasts them over rows
+            assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
+            edges = edges.unsqueeze(1).expand(b, n, n)
+        graph = self._sparse_graph if any(_is_sparse(t) for t in (adj_mat, edges, neighbor_mask)) else self._dense_graph
+        idx, nmask, rel_pos, rel_dist, e = graph(coors, mask, adj_mat, edges, neighbor_mask, b, n, valid_radius)
 
         pos_emb = None
         if exists(self.rotary_pos_emb):
@@ -1555,11 +1531,43 @@ class SE3Transformer(nn.Module):
 
         return adj_indices, sparse_mask, num_sparse
 
+    def _valid_radius(self):
+        """The search radius: none at all when only bonded neighbours are attended to (num_neighbors == 0)."""
+        assert self.attend_sparse_neighbors or self.num_neighbors > 0, 'you must either attend to sparsely bonded neighbors, or set number of locally attended neighbors to be greater than 0'
+        return 0 if self.num_neighbors == 0 else self.valid_radius
+
     def _num_neighbors(self, n, num_sparse):
         """Neighbour slots per node: the local neighbours plus the bonded ones, at most n - 1 (reference S:1220-1226)."""
         total = int(int(min(self.num_neighbors, n - 1)) + num_sparse)
         assert total > 0, 'you must be fetching at least 1 neighbor'
         return int(min(total, n - 1))
+
+    def _edge_features(self, edge_values, hop_values):
+        """Edge features on the neighbour list (reference S:1231-1239, 1293-1294) from the pair values each graph builder looked
+        up on it: edge tokens embedded or continuous edges as float, then the embedded hop counts concatenated; None if neither."""
+        e = None
+        if edge_values is not None:
+            e = self.edge_emb(edge_values) if exists(self.edge_emb) else edge_values.float()
+        if hop_values is not None:
+            a = self.adj_emb(hop_values)
+            e = torch.cat((e, a), dim=-1) if exists(e) else a
+        return e
+
+    def _dense_graph(self, coors, mask, adj_mat, edges, neighbor_mask, b, n, valid_radius):
+        """The neighbour graph and edge features of _forward_once with dense pair inputs: the search reads the byte masks, and
+        edge values and hop counts are gathered on the neighbour list (gather first, embed after).  Returns idx, nmask,
+        rel_pos, rel_dist, e."""
+        adj_indices, sparse_mask, num_sparse = self._bonded(adj_mat, b, n, coors.device)
+        if exists(neighbor_mask):
+            eye = torch.eye(n, dtype=torch.bool, device=neighbor_mask.device)
+            self._report_neighbor_mask(neighbor_mask.masked_fill(eye.unsqueeze(0), False).sum(dim=-1))
+        idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), self._num_neighbors(n, num_sparse), valid_radius, node_mask=mask,
+                                                neighbor_mask=neighbor_mask, sparse_adj=sparse_mask, causal=self.causal)
+        edge_values = None
+        if exists(edges):
+            edge_values = edges.gather(2, idx) if exists(self.edge_emb) else ops.gather_pairs(edges.float(), idx)
+        hops = adj_indices.gather(2, idx) if exists(self.adj_emb) else None
+        return idx, nmask, rel_pos, rel_dist, self._edge_features(edge_values, hops)
 
     # ---- sparse pair inputs --------------------------------------------------------------------------------
     def _check_sparse_pairs(self, coors, adj_mat, edges, neighbor_mask):
@@ -1660,7 +1668,7 @@ class SE3Transformer(nn.Module):
 
     def _sparse_graph(self, coors, mask, adj_mat, edges, neighbor_mask, b, n, valid_radius):
         """The neighbour graph and edge features of _forward_once when at least one pair input is torch.sparse_coo (the dense
-        ones are converted): the search reads sorted column lists (ops.knn_csr), and edge tokens, edge features and hop counts
+        ones are converted): the search reads sorted column lists (ops.PairRows), and edge tokens, edge features and hop counts
         are looked up in them (ops.pair_lookup).  Memory is O(nnz + n k).  Returns idx, nmask, rel_pos, rel_dist, e."""
         hops, bonded, num_sparse = None, None, 0
         if exists(self.num_adj_degrees) or self.attend_sparse_neighbors:
@@ -1676,27 +1684,17 @@ class SE3Transformer(nn.Module):
             self._report_neighbor_mask(torch.zeros(nbr.ptr.numel() - 1, dtype=dt, device=v.device).index_add_(0, rows[off], v[off].to(dt)))
             allowed = v if v.dtype == torch.bool else v.to(torch.uint8) != 0              # the byte the dense search reads
             nbr = ops.pair_rows(rows[allowed], nbr.cols[allowed], v[allowed], nbr.ptr.numel() - 1, nbr.shared)
-        idx, nmask, rel_pos, rel_dist = ops.knn_csr(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=nbr,
-                                                    bonded=bonded, causal=self.causal)
+        idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), total, valid_radius, node_mask=mask, neighbor_mask=nbr,
+                                                sparse_adj=bonded, causal=self.causal)
 
         def lookup(rows):
             """rows.values on the neighbour list, zero where a pair is absent"""
             v = rows.values
             return torch.cat((v, v.new_zeros((1, *v.shape[1:]))))[ops.pair_lookup(rows, idx)]
 
-        e = None
-        if exists(edges):
-            if not edges.is_sparse:
-                if exists(self.edge_emb) and edges.dim() == 2:  # [b, n] tokens: the reference broadcasts them over rows (b == 1)
-                    assert b == 1, 'edges of shape [b, n] only broadcast for batch size 1 (as in the reference)'
-                    edges = edges.unsqueeze(1).expand(b, n, n)
-                edges = edges.to_sparse(3)
-            pairs = ops.coo_to_rows(edges, n)
-            e = self.edge_emb(lookup(pairs)) if exists(self.edge_emb) else lookup(pairs._replace(values=pairs.values.float()))
-        if exists(self.adj_emb):
-            a = self.adj_emb(lookup(hops))
-            e = torch.cat((e, a), dim=-1) if exists(e) else a
-        return idx, nmask, rel_pos, rel_dist, e
+        edge_values = lookup(ops.coo_to_rows(edges if edges.is_sparse else edges.to_sparse(3), n)) if exists(edges) else None
+        hop_values = lookup(hops) if exists(self.adj_emb) else None
+        return idx, nmask, rel_pos, rel_dist, self._edge_features(edge_values, hop_values)
 
     def _report_neighbor_mask(self, row_counts):
         """Reference S:1253: row_counts [...] are the row sums of neighbor_mask without its diagonal."""
@@ -1814,18 +1812,13 @@ class SE3Transformer(nn.Module):
             feats = self._embed_tokens(feats.unsqueeze(0), local_pos)
             feats = {'0': feats[..., None]}
         feats = self._check_features(feats, coors)
-        neighbors, valid_radius = self.num_neighbors, self.valid_radius
-        assert self.attend_sparse_neighbors or neighbors > 0, 'you must either attend to sparsely bonded neighbors, or set number of locally attended neighbors to be greater than 0'
-        if neighbors == 0:
-            valid_radius = 0
+        valid_radius = self._valid_radius()
 
         # per cloud, exactly as forward() on that cloud alone: bonded neighbours, hop counts and the neighbour count k_c
         ks, sparse, hops = [], [], []
         for c, n in enumerate(seqlens):
             adj_indices, sparse_mask, num_sparse = self._bonded(adj_mat[c].to(dev) if exists(adj_mat) else None, 1, n, dev)
-            total = int(int(min(neighbors, n - 1)) + num_sparse)
-            assert total > 0, 'you must be fetching at least 1 neighbor'
-            ks.append(int(min(total, n - 1)))
+            ks.append(self._num_neighbors(n, num_sparse))
             if exists(sparse_mask):
                 sparse.append(sparse_mask.reshape(-1))
             if exists(adj_indices):
@@ -1834,19 +1827,15 @@ class SE3Transformer(nn.Module):
                 eye = torch.eye(n, dtype=torch.bool, device=dev)
                 self._report_neighbor_mask(neighbor_mask[c].to(dev).masked_fill(eye, False).sum(dim=-1))
         nbr = torch.cat([m.to(dev).reshape(-1) for m in neighbor_mask]) if exists(neighbor_mask) else None
-        idx, nmask, rel_pos, rel_dist = ops.knn_varlen(coors.float(), seqlens, ks, max(ks), valid_radius, neighbor_mask=nbr,
-                                                       sparse_adj=torch.cat(sparse) if sparse else None, causal=self.causal)
+        idx, nmask, rel_pos, rel_dist = ops.knn(coors.float(), ks, valid_radius, neighbor_mask=nbr,
+                                                sparse_adj=torch.cat(sparse) if sparse else None, causal=self.causal, seqlens=seqlens)
 
-        # edge features: pair (i, j) of cloud c sits at pair_off[c] + i_local n_c + j_local of the flattened per-cloud inputs
-        e = None
-        if exists(edges) or exists(self.adj_emb):
-            flat = pair_row.to(dev)[:, None] + idx                                      # [T, K]
+        # edge values: pair (i, j) of cloud c sits at pair_off[c] + i_local n_c + j_local of the flattened per-cloud inputs
+        flat = pair_row.to(dev)[:, None] + idx if exists(edges) or exists(self.adj_emb) else None      # [T, K]
+        edge_values = None
         if exists(edges):
-            pf = torch.cat([t.to(dev).reshape(n * n, *t.shape[2:]) for t, n in zip(edges, seqlens)])
-            e = self.edge_emb(pf[flat]) if exists(self.edge_emb) else pf.float()[flat]
-        if exists(self.adj_emb):
-            a = self.adj_emb(torch.cat(hops)[flat])
-            e = torch.cat((e, a), dim=-1) if exists(e) else a
+            edge_values = torch.cat([t.to(dev).reshape(n * n, *t.shape[2:]) for t, n in zip(edges, seqlens)])[flat]
+        e = self._edge_features(edge_values, torch.cat(hops)[flat] if exists(self.adj_emb) else None)
 
         idx, nmask, rel_pos, rel_dist = idx.unsqueeze(0), nmask.unsqueeze(0), rel_pos.unsqueeze(0), rel_dist.unsqueeze(0)
         pos_emb = None

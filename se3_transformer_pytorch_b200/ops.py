@@ -23,10 +23,7 @@ c_void_p, c_int, c_int64, c_float = ctypes.c_void_p, ctypes.c_int, ctypes.c_int6
 _SIGNATURES = {
     'se3_last_error': (ctypes.c_char_p, []),
     'se3_abi_version': (c_int, []),
-    'se3_knn_fwd': (c_int, [c_void_p] * 4 + [c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
-    'se3_knn_varlen_fwd': (c_int, [c_void_p] * 6 + [c_int, c_int64, c_int, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
-    'se3_knn_csr_fwd': (c_int, [c_void_p] * 4 + [c_int64, c_int64] + [c_void_p] * 2 + [c_int64, c_int64, c_int, c_int, c_int, c_float, c_int]
-                        + [c_void_p] * 4 + [c_void_p]),
+    'se3_knn_fwd': (c_int, [c_void_p] * 7 + [c_int, c_int64, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
     'se3_pair_lookup_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
@@ -140,43 +137,9 @@ def _u8(t):
 # ---------------------------------------------------------------------------------------------------------
 # K1
 # ---------------------------------------------------------------------------------------------------------
-def knn(coors, k, valid_radius, node_mask=None, neighbor_mask=None, sparse_adj=None, causal=False):
-    """Neighbour graph (reference se3_transformer_pytorch.py:1171-1294).
-    Returns idx int64 [b,n,k], mask bool [b,n,k], rel_pos [b,n,k,3], rel_dist [b,n,k]."""
-    _require_cuda(coors, node_mask, neighbor_mask, sparse_adj)
-    coors = _f32(coors)
-    b, n, _ = coors.shape
-    # the kernel indexes the masks as [b, n] / [b, n, n]: broadcastable inputs ([n, n], [1, n, n]) are expanded here, anything
-    # else is refused instead of being read out of bounds
-    if node_mask is not None:
-        if node_mask.shape != (b, n):
-            raise ValueError(f'knn: node_mask must be [b, n] = {(b, n)}, got {tuple(node_mask.shape)}')
-    pair = []
-    for name, t in (('neighbor_mask', neighbor_mask), ('sparse_adj', sparse_adj)):
-        if t is not None:
-            if t.dim() == 2:
-                t = t.unsqueeze(0)
-            if t.shape[-2:] != (n, n) or t.shape[0] not in (1, b):
-                raise ValueError(f'knn: {name} must be [n, n], [1, n, n] or [b, n, n] with b, n = {(b, n)}, got {tuple(t.shape)}')
-            t = t.expand(b, n, n)
-        pair.append(t)
-    neighbor_mask, sparse_adj = pair
-    idx = torch.empty((b, n, k), dtype=torch.int64, device=coors.device)
-    mask = torch.empty((b, n, k), dtype=torch.uint8, device=coors.device)
-    rel_pos = torch.empty((b, n, k, 3), dtype=torch.float32, device=coors.device)
-    rel_dist = torch.empty((b, n, k), dtype=torch.float32, device=coors.device)
-    nm, nbm, sa = _u8(node_mask), _u8(neighbor_mask), _u8(sparse_adj)
-    valid_radius = float(min(valid_radius, 3.0e38))
-    nbytes = 12 * b * n + 25 * b * n * k + sum(t.numel() for t in (nm, nbm, sa) if t is not None)
-    with torch.cuda.device(coors.device), _timed('knn', nbytes=nbytes):
-        _check(lib().se3_knn_fwd(_p(coors), _p(nm), _p(nbm), _p(sa), b, n, k, valid_radius, int(bool(causal)),
-                                 _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
-    return idx, mask.view(torch.bool), rel_pos, rel_dist
-
-
 class PairRows(NamedTuple):
-    """A sparse pair input in the row format of se3_knn_csr_fwd: row r = b * n + i (or i when shared) holds entries
-    ptr[r] .. ptr[r+1] of cols (ascending, unique) and values."""
+    """A sparse pair input as sorted column lists (se3_pairs of se3_knn_fwd): row r = b * n + i (or i when shared) holds
+    entries ptr[r] .. ptr[r+1] of cols (ascending, unique) and values."""
     ptr: torch.Tensor         # int64 [rows + 1]
     cols: torch.Tensor        # int32 [nnz], node index inside the cloud
     values: torch.Tensor      # [nnz, ...] in the input's dtype
@@ -206,40 +169,12 @@ def coo_to_rows(t, n):
 def _row_args(rows, b, n):
     """(ptr, cols, nnz, batch stride) of a PairRows for a batch [b, n]; an empty list keeps a non-NULL column pointer, since
     NULL means no list."""
-    if rows is None:
-        return None, None, 0, 0
     want = (n if rows.shared else b * n) + 1
     if rows.ptr.dtype != torch.int64 or rows.ptr.shape != (want,) or rows.cols.dtype != torch.int32 or rows.cols.dim() != 1:
         raise ValueError(f'pair rows for b, n = {(b, n)} need int64 row pointers [{want}] and int32 columns [nnz], got '
                          f'{rows.ptr.dtype} {tuple(rows.ptr.shape)} and {rows.cols.dtype} {tuple(rows.cols.shape)}')
     cols = rows.cols.contiguous() if rows.cols.numel() else torch.zeros(1, dtype=torch.int32, device=rows.cols.device)
     return rows.ptr.contiguous(), cols, rows.cols.numel(), 0 if rows.shared else n
-
-
-def knn_csr(coors, k, valid_radius, node_mask=None, neighbor_mask=None, bonded=None, causal=False):
-    """knn() with the pair masks given as PairRows: neighbor_mask lists the allowed columns of each row, bonded the bonded
-    ones.  Bit-identical to knn() on the densified masks.  Returns idx int64 [b,n,k], mask bool [b,n,k], rel_pos [b,n,k,3],
-    rel_dist [b,n,k]."""
-    _require_cuda(coors, node_mask, *(r.ptr for r in (neighbor_mask, bonded) if r is not None),
-                  *(r.cols for r in (neighbor_mask, bonded) if r is not None))
-    coors = _f32(coors)
-    b, n, _ = coors.shape
-    if node_mask is not None and node_mask.shape != (b, n):
-        raise ValueError(f'knn_csr: node_mask must be [b, n] = {(b, n)}, got {tuple(node_mask.shape)}')
-    nptr, ncols, nnnz, nstride = _row_args(neighbor_mask, b, n)
-    aptr, acols, annz, astride = _row_args(bonded, b, n)
-    idx = torch.empty((b, n, k), dtype=torch.int64, device=coors.device)
-    mask = torch.empty((b, n, k), dtype=torch.uint8, device=coors.device)
-    rel_pos = torch.empty((b, n, k, 3), dtype=torch.float32, device=coors.device)
-    rel_dist = torch.empty((b, n, k), dtype=torch.float32, device=coors.device)
-    nm = _u8(node_mask)
-    valid_radius = float(min(valid_radius, 3.0e38))
-    nbytes = 12 * b * n + 25 * b * n * k + (0 if nm is None else nm.numel()) + 4 * (nnnz + annz)
-    with torch.cuda.device(coors.device), _timed('knn', nbytes=nbytes):
-        _check(lib().se3_knn_csr_fwd(_p(coors), _p(nm), _p(nptr), _p(ncols), nnnz, nstride, _p(aptr), _p(acols), annz, astride,
-                                     b, n, k, valid_radius, int(bool(causal)), _p(idx), _p(mask), _p(rel_pos), _p(rel_dist),
-                                     _stream()))
-    return idx, mask.view(torch.bool), rel_pos, rel_dist
 
 
 def pair_lookup(rows, idx):
@@ -265,41 +200,77 @@ def pair_offsets(seqlens):
     return off
 
 
-def knn_varlen(coors, seqlens, k_per_cloud, K, valid_radius, neighbor_mask=None, sparse_adj=None, causal=False):
-    """Neighbour graph of a packed batch (SE3Transformer.forward_packed): clouds of seqlens[c] nodes laid end to end in
-    coors [T, 3], each searched on its own for k_per_cloud[c] neighbours, K >= max k_c slots per node (slots past k_c repeat
-    slot k_c - 1, masked).  neighbor_mask / sparse_adj: the clouds' [n_c, n_c] matrices flattened end to end ([sum n_c^2]).
-    Returns idx int64 [T, K] (global node indices), mask bool [T, K], rel_pos [T, K, 3], rel_dist [T, K]."""
-    _require_cuda(coors, neighbor_mask, sparse_adj)
+class _Pairs(ctypes.Structure):
+    _fields_ = [('dense', c_void_p), ('row_ptr', c_void_p), ('cols', c_void_p), ('nnz', c_int64), ('shared', c_int)]
+
+
+def knn(coors, k, valid_radius, *, node_mask=None, neighbor_mask=None, sparse_adj=None, causal=False, seqlens=None, K=None):
+    """Neighbour graph (reference se3_transformer_pytorch.py:1171-1294) of a padded or a packed batch.
+    Padded: coors [b, n, 3], k neighbours of every node, node_mask [b, n].  Returns idx int64 [b, n, k] (indices inside the
+    cloud), mask bool [b, n, k], rel_pos [b, n, k, 3], rel_dist [b, n, k].
+    Packed (SE3Transformer.forward_packed): clouds of seqlens[c] nodes laid end to end in coors [T, 3], each searched on its
+    own for k[c] neighbours, K >= max k_c slots per node (default max k_c; slots past k_c repeat slot k_c - 1, masked).
+    Returns idx int64 [T, K] (global node indices), mask bool [T, K], rel_pos [T, K, 3], rel_dist [T, K].
+    neighbor_mask / sparse_adj: a tensor ([n, n], [1, n, n] or [b, n, n] padded; the clouds' [n_c, n_c] matrices flattened end
+    to end when packed) or, padded only, a PairRows; the two give the same results bit for bit."""
+    pair_inputs = [t for t in (neighbor_mask, sparse_adj) if t is not None]
+    _require_cuda(coors, node_mask, *(x for t in pair_inputs for x in (t[:2] if isinstance(t, PairRows) else (t,))))
     coors = _f32(coors)
-    seqlens, k_per_cloud = [int(v) for v in seqlens], [int(v) for v in k_per_cloud]
-    B, T = len(seqlens), sum(seqlens)
-    if B == 0 or coors.shape != (T, 3):
-        raise ValueError(f'knn_varlen: coors must be [sum(seqlens), 3] = {(T, 3)} for {B} clouds, got {tuple(coors.shape)}')
-    if len(k_per_cloud) != B:
-        raise ValueError(f'knn_varlen: k_per_cloud has {len(k_per_cloud)} entries for {B} clouds')
-    if min(seqlens) < 2 or max(seqlens) > MAX_CLOUD:
-        raise ValueError(f'knn_varlen: every cloud needs 2 .. {MAX_CLOUD} nodes, got lengths {min(seqlens)} .. {max(seqlens)}')
-    if any(not 1 <= kc <= n - 1 for kc, n in zip(k_per_cloud, seqlens)) or K < max(k_per_cloud):
-        raise ValueError(f'knn_varlen: need 1 <= k_c <= n_c - 1 and K >= max k_c (K = {K}, k = {k_per_cloud}, n = {seqlens})')
-    npairs = sum(n * n for n in seqlens)
-    for name, t in (('neighbor_mask', neighbor_mask), ('sparse_adj', sparse_adj)):
-        if t is not None and t.shape != (npairs,):
-            raise ValueError(f'knn_varlen: {name} must be the flattened per-cloud [n_c, n_c] matrices, [{npairs}], got {tuple(t.shape)}')
     dev = coors.device
-    cu = torch.tensor([0] + seqlens, dtype=torch.int64).cumsum(0).to(dev)
-    kc = torch.tensor(k_per_cloud, dtype=torch.int32).to(dev)
-    nbm, sa = _u8(neighbor_mask), _u8(sparse_adj)
-    off = torch.tensor(pair_offsets(seqlens), dtype=torch.int64).to(dev) if nbm is not None or sa is not None else None
-    idx = torch.empty((T, K), dtype=torch.int64, device=dev)
-    mask = torch.empty((T, K), dtype=torch.uint8, device=dev)
-    rel_pos = torch.empty((T, K, 3), dtype=torch.float32, device=dev)
-    rel_dist = torch.empty((T, K), dtype=torch.float32, device=dev)
+    cu = kc = off = None
+    if seqlens is None:
+        b, n, _ = coors.shape
+        T, K = b * n, k
+        if node_mask is not None and node_mask.shape != (b, n):
+            raise ValueError(f'knn: node_mask must be [b, n] = {(b, n)}, got {tuple(node_mask.shape)}')
+    else:
+        seqlens, k = [int(v) for v in seqlens], [int(v) for v in k]
+        b, T = len(seqlens), sum(seqlens)
+        n = T                                       # se3_knn_fwd takes the number of all nodes here
+        if b == 0 or coors.shape != (T, 3):
+            raise ValueError(f'knn: coors must be [sum(seqlens), 3] = {(T, 3)} for {b} clouds, got {tuple(coors.shape)}')
+        if len(k) != b:
+            raise ValueError(f'knn: k has {len(k)} entries for {b} clouds')
+        if min(seqlens) < 2 or max(seqlens) > MAX_CLOUD:
+            raise ValueError(f'knn: every cloud needs 2 .. {MAX_CLOUD} nodes, got lengths {min(seqlens)} .. {max(seqlens)}')
+        K = max(k) if K is None else K
+        if any(not 1 <= k_c <= n_c - 1 for k_c, n_c in zip(k, seqlens)) or K < max(k):
+            raise ValueError(f'knn: need 1 <= k_c <= n_c - 1 and K >= max k_c (K = {K}, k = {k}, n = {seqlens})')
+        cu = torch.tensor([0] + seqlens, dtype=torch.int64).cumsum(0).to(dev)
+        kc = torch.tensor(k, dtype=torch.int32).to(dev)
+        if any(torch.is_tensor(t) for t in pair_inputs):
+            off = torch.tensor(pair_offsets(seqlens), dtype=torch.int64).to(dev)
+    nm = _u8(node_mask)
+    keep, args, nbytes = [], [], 12 * T + 25 * T * K + (0 if nm is None else nm.numel())
+    for name, t in (('neighbor_mask', neighbor_mask), ('sparse_adj', sparse_adj)):
+        if t is None:
+            args.append(None)
+            continue
+        if isinstance(t, PairRows):
+            ptr, cols, nnz, stride = _row_args(t, T // n, n)   # (packed clouds refuse column lists)
+            keep += [ptr, cols]
+            args.append(ctypes.byref(_Pairs(None, _p(ptr), _p(cols), nnz, int(stride == 0))))
+            nbytes += 4 * nnz
+            continue
+        if seqlens is not None:
+            npairs = sum(n_c * n_c for n_c in seqlens)
+            if t.shape != (npairs,):
+                raise ValueError(f'knn: {name} must be the flattened per-cloud [n_c, n_c] matrices, [{npairs}], got {tuple(t.shape)}')
+        elif t.shape[-2:] != (n, n) or t.dim() not in (2, 3) or (t.dim() == 3 and t.shape[0] not in (1, b)):
+            raise ValueError(f'knn: {name} must be [n, n], [1, n, n] or [b, n, n] with b, n = {(b, n)}, got {tuple(t.shape)}')
+        t = _u8(t)
+        keep.append(t)
+        args.append(ctypes.byref(_Pairs(_p(t), None, None, 0, int(seqlens is None and (t.dim() == 2 or t.shape[0] == 1)))))
+        nbytes += t.numel()
+    rows = (T, K) if seqlens is not None else (b, n, K)
+    idx = torch.empty(rows, dtype=torch.int64, device=dev)
+    mask = torch.empty(rows, dtype=torch.uint8, device=dev)
+    rel_pos = torch.empty((*rows, 3), dtype=torch.float32, device=dev)
+    rel_dist = torch.empty(rows, dtype=torch.float32, device=dev)
     valid_radius = float(min(valid_radius, 3.0e38))
-    nbytes = 12 * T + 25 * T * K + sum(t.numel() for t in (nbm, sa) if t is not None)
-    with torch.cuda.device(dev), _timed('knn_varlen', nbytes=nbytes):
-        _check(lib().se3_knn_varlen_fwd(_p(coors), _p(cu), _p(kc), _p(nbm), _p(sa), _p(off), B, T, K, max(seqlens), valid_radius,
-                                        int(bool(causal)), _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
+    with torch.cuda.device(dev), _timed('knn' if seqlens is None else 'knn_varlen', nbytes=nbytes):
+        _check(lib().se3_knn_fwd(_p(coors), _p(cu), _p(kc), _p(off), _p(nm), *args, b, n, K, valid_radius, int(bool(causal)),
+                                 _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
     return idx, mask.view(torch.bool), rel_pos, rel_dist
 
 

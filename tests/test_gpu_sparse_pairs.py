@@ -1,6 +1,6 @@
 """Sparse pair inputs of SE3Transformer.forward on the GPU:
 
-  * ops.knn_csr, the neighbour search reading sorted column lists, against ops.knn on the densified masks, bit for bit, on the
+  * ops.knn reading sorted column lists (ops.PairRows) against ops.knn on the densified masks, bit for bit, on the
     cases of the tiled-search test plus empty rows, an empty neighbour list and a batch-shared 2-D adjacency;
   * ops.pair_lookup against the dense gathers, -1 for absent pairs;
   * every reference fixture with pair inputs, run with them as torch.sparse_coo (also uncoalesced, with stored zeros): bit for bit
@@ -34,7 +34,7 @@ CSR_CASES = KNN_CASES + [
 
 
 @pytest.mark.parametrize('case', CSR_CASES, ids=lambda c: '-'.join(f'{k}{v}' for k, v in c.items()))
-def test_knn_csr_matches_dense_knn_bit_for_bit(case):
+def test_knn_column_lists_match_dense_masks_bit_for_bit(case):
     from se3_transformer_pytorch_b200 import ops
     rng = np.random.default_rng(case['n'] + case['k'])
     b, n = case.get('b', 1), case['n']
@@ -67,7 +67,7 @@ def test_knn_csr_matches_dense_knn_bit_for_bit(case):
     rows = lambda t: None if t is None else ops.coo_to_rows(t.to_sparse(), n)
     if adj is not None and case.get('shared'):
         assert rows(adj_t).shared
-    sparse = ops.knn_csr(cu(coors), k, radius, neighbor_mask=rows(nbr_t), bonded=rows(adj_t), **kw)
+    sparse = ops.knn(cu(coors), k, radius, neighbor_mask=rows(nbr_t), sparse_adj=rows(adj_t), **kw)
     for a, s in zip(dense, sparse):
         assert torch.equal(a, s)
 

@@ -1,4 +1,4 @@
-"""Packed batches of clouds of different sizes on the GPU (SE3Transformer.forward_packed, ops.knn_varlen): the segmented neighbour
+"""Packed batches of clouds of different sizes on the GPU (SE3Transformer.forward_packed, ops.knn with seqlens): the segmented neighbour
 search against the padded one per cloud (bit for bit), the whole model against the real reference run once per cloud and against a
 per-cloud loop of forward(), equivariance per cloud, independence of the clouds and the edge count."""
 import numpy as np
@@ -36,7 +36,7 @@ KNN_CASES = [
 
 
 @pytest.mark.parametrize('case', KNN_CASES, ids=lambda c: ','.join(f'{k}={v if k != "lens" else len(v)}' for k, v in c.items()))
-def test_knn_varlen_matches_padded_knn_per_cloud(case):
+def test_knn_packed_matches_padded_knn_per_cloud(case):
     from se3_transformer_pytorch_b200 import ops
     lens, k = case['lens'], case['k']
     g = torch.Generator().manual_seed(5)
@@ -47,7 +47,8 @@ def test_knn_varlen_matches_padded_knn_per_cloud(case):
     ks = [min(k + (int(a.sum(-1).max()) if adj else 0), n - 1) for n, a in zip(lens, adj or [None] * len(lens))]
     flat = lambda ms: None if ms is None else torch.cat([m.reshape(-1) for m in ms]).to(DEV)
     K = max(ks)
-    idx, mask, rel_pos, rel_dist = ops.knn_varlen(coors, lens, ks, K, radius, neighbor_mask=flat(nbr), sparse_adj=flat(adj), causal=causal)
+    idx, mask, rel_pos, rel_dist = ops.knn(coors, ks, radius, neighbor_mask=flat(nbr), sparse_adj=flat(adj), causal=causal, seqlens=lens,
+                                           K=K)
     assert idx.shape == (sum(lens), K) and rel_pos.shape == (sum(lens), K, 3)
     s = 0
     for c, (n, kc) in enumerate(zip(lens, ks)):

@@ -27,9 +27,9 @@ def test_state_dict_layout_matches_reference_high_degree(name):
     test_state_dict_layout_matches_reference(name)
 
 
-def test_library_matches_header_at_abi_version_2():
-    """The C-ABI library loads on a GPU-less box, exports everything include/se3b200.h declares and reports ABI version 2
-    (se3_linear_tc_fwd takes flush_stages; the strided low-rank entry point is gone)."""
+def test_library_matches_header_at_abi_version_3():
+    """The C-ABI library loads on a GPU-less box, exports everything include/se3b200.h declares and reports ABI version 3
+    (one se3_knn_fwd for uniform and packed clouds and for dense and column-list pair masks)."""
     from se3_transformer_pytorch_b200 import build, ops
     path = build.build()
     handle = ctypes.CDLL(path)
@@ -39,7 +39,7 @@ def test_library_matches_header_at_abi_version_2():
     for sym in declared:
         assert hasattr(handle, sym), f'{sym} declared in se3b200.h but not exported'
     assert declared == set(ops.EXPORTED_SYMBOLS)
-    assert ops.lib().se3_abi_version() == 2
+    assert ops.lib().se3_abi_version() == 3
 
 
 def test_build_stamp_survives_a_move_of_the_tree(tmp_path):
