@@ -480,25 +480,16 @@ class ConvSE3(nn.Module):
         return feat.reshape(-1, feat.shape[-1]).contiguous()
 
     def forward(self, inp, edge_info, rel_dist=None, basis=None):
-        geom = basis[2] if isinstance(basis, tuple) and len(basis) > 2 else None
-        if not self.pool or geom is None or geom.edge_budget is None:
-            return conv_forward([self], inp, edge_info, rel_dist, basis)[0]
-        # node chunks under the edge budget: the pooled outputs of every chunk land in their rows of the node-level result
-        decisions = [conv_decide(self, edge_info[0].numel(), rel_dist, geom, torch.cuda.is_current_stream_capturing())]
-        chunks = geom.node_chunks(decisions, edge_info[0].shape)
-        if len(chunks) == 1:
-            return conv_forward([self], inp, edge_info, rel_dist, basis, decisions=decisions)[0]
-        self_out = self.self_interact(inp) if self.self_interaction else None
-        sx = chunk_edge_scale(decisions, inp, edge_info[0])
-        b, n = edge_info[0].shape[:2]
-        out = {str(do): torch.empty((b, n, mo, to_order(do)), dtype=torch.float32, device=rel_dist.device)
-               for do, mo in self.fiber_out}
-        for c in chunks:
-            res = conv_forward([self], c.src(inp), c.edge_info(edge_info), c.rows(rel_dist), (None, None, geom.chunk(c)),
-                               decisions=decisions, self_out=c.rows(self_out), sx=c.rows(sx))[0]
-            for d, t in res.items():
-                c.rows(out[d]).copy_(t)
-        return out
+        flat, plan, geom = split_basis(basis)
+        decisions = [conv_decide(self, edge_info[0].numel(), rel_dist, geom)]
+        whole_self = {}          # node chunks add their rows of the whole graph's self-interaction, made for the first of them
+
+        def evaluate(c, cbasis, sx):
+            if not c.whole and self.self_interaction and not whole_self:
+                whole_self.update(self.self_interact(inp))
+            return conv_forward([self], c.src(inp), c.edge_info(edge_info), c.rows(rel_dist), cbasis, decisions=decisions,
+                                self_out=c.rows(whole_self) if whole_self else None, sx=sx)[0]
+        return over_node_chunks((flat, plan, geom), decisions, inp, edge_info[0], evaluate)
 
 
 def input_side(di, do):
@@ -516,18 +507,19 @@ def lowrank_k(r):
 class Geometry:
     """Per-forward edge geometry shared by every layer; the aligned frames and the flat basis are built on first use, the frames
     by the code that the host_frames switch selects when the Geometry is made.  chunk() gives the Geometry of the edges of one
-    node chunk (NodeChunk), which builds its own frames and basis and shares the whole graph's d_max and deferred checks."""
+    node chunk (NodeChunk), which builds its own frames and basis and shares the whole graph's d_max and deferred checks.
 
-    def __init__(self, rel_pos, max_degree, whole=None):
+    deferred: where the run-time checks of the low-rank plans go, as (ConvSE3, stats [pairs, 2], have): None = check inside
+    every ConvSE3 (one host synchronisation each); a list = the caller collects them and checks once per forward
+    (SE3Transformer.forward).  edge_budget: bytes the edge-level tensors of one block may take (edge_budget_bytes), or None:
+    every block runs as one chunk."""
+
+    def __init__(self, rel_pos, max_degree, deferred=None, edge_budget=None, whole=None):
         self.rel_pos, self.max_degree, self._frames, self._basis = rel_pos, max_degree, None, None
+        self.deferred, self.edge_budget = deferred, edge_budget
         self.whole = self if whole is None else whole
         self.host_frames = switches.current().host_frames if whole is None else whole.host_frames
-        # run-time checks of the low-rank plans, as (ConvSE3, stats [pairs, 2]) : None = check inside every ConvSE3 (one host
-        # synchronisation each); a list = the caller collects them and checks once per forward (SE3Transformer.forward)
-        self.deferred = None if whole is None else whole.deferred
         self._dmax = None
-        # bytes the edge-level tensors of one block may take (edge_budget_bytes), or None: every block runs as one chunk
-        self.edge_budget = None
 
     def d_max(self, rel_dist):
         if self is not self.whole:
@@ -540,13 +532,7 @@ class Geometry:
         """The Geometry of the edges of node chunk c (self when c is the whole graph)."""
         if c.whole:
             return self
-        return Geometry(c.rows(self.rel_pos), self.max_degree, whole=self)
-
-    def node_chunks(self, decisions, shape, keep_aligned=False, attn_bytes=0):
-        """The node chunks of one block of the graph idx [b, n, k] = shape: one chunk without an edge budget."""
-        b, n, k = shape
-        per_edge = block_edge_bytes(decisions, self.max_degree, keep_aligned, attn_bytes)
-        return plan_node_chunks(b, n, k, per_edge, self.whole.edge_budget)
+        return Geometry(c.rows(self.rel_pos), self.max_degree, self.deferred, self.edge_budget, whole=self)
 
     def basis(self):
         """(flat basis buffer, BasisPlan) of these edges (ops.basis_flat), for the R-first route."""
@@ -705,6 +691,30 @@ def chunk_edge_scale(decisions, inp, idx):
     return ops.edge_scale(inp, idx, max(di for di, _ in decisions[0].conv.fiber_in)).view(idx.shape)
 
 
+def over_node_chunks(basis, decisions, inp, idx, evaluate, keep_aligned=False, attn_bytes=0):
+    """The edge work of one block -- the convolutions of `decisions` on the graph idx [b, n, k] with node features inp -- over
+    the node chunks that the edge budget of the block's Geometry allows (DESIGN.md 4.7); basis: (flat, BasisPlan, Geometry or
+    None).  evaluate(c, chunk basis, sx) gives the outputs {key: [b', n', ...]} of NodeChunk c; sx: c's rows of the whole
+    graph's edge scales (chunk_edge_scale).  The whole graph (one chunk, also without a Geometry or a budget) gets the block's
+    basis and sx None, and its outputs are returned as they are; otherwise each chunk gets its own Geometry and its outputs
+    land in their rows of [b, n, ...] tensors."""
+    _, _, geom = basis
+    b, n, k = idx.shape
+    per_edge = 0 if geom is None else block_edge_bytes(decisions, geom.max_degree, keep_aligned, attn_bytes)
+    chunks = plan_node_chunks(b, n, k, per_edge, None if geom is None else geom.edge_budget)
+    if len(chunks) == 1:
+        return evaluate(chunks[0], basis, None)
+    sx = chunk_edge_scale(decisions, inp, idx)
+    out = None
+    for c in chunks:
+        res = evaluate(c, (None, None, geom.chunk(c)), c.rows(sx))
+        if out is None:
+            out = {key: t.new_empty((b, n) + t.shape[2:]) for key, t in res.items()}
+        for key, t in res.items():
+            c.rows(out[key]).copy_(t)
+    return out
+
+
 class ConvDecision:
     """What one ConvSE3 decides once per forward, from the whole graph (conv_decide): the switches sw, tc_ok {pair: bool}, the
     low-rank plan or None, its covered pairs lr and the route they give, whether direct kernels need g, and the stats
@@ -719,18 +729,25 @@ class ConvDecision:
 
 
 class ConvDispatch:
-    """How one ConvSE3 runs in one forward (conv_dispatch).  route: 'production' (DESIGN.md 4.5, GEMM images z), 'aligned' (4.4)
-    or 'rfirst' (4.1-4.3, with each pair's kernel in how: 'input_side', 'combined', 'tc' or 'simt').  U [pairs, E, 64]: radial
-    coordinates of the low-rank pairs lr = {pair: plan entry}; g [pairs, E, 128]: trunk outputs for the direct kernels.  Outputs
-    go to outs {do: [E, Co, 2do+1]}, or on the production route to pooled or aligned_out.  sw: the switches of this forward."""
+    """How one ConvSE3 runs on one set of edges (conv_dispatch) under its decision d (ConvDecision), which gives conv, sw, plan,
+    route and lr.  route: 'production' (DESIGN.md 4.5, GEMM images plan['z']), 'aligned' (4.4) or 'rfirst' (4.1-4.3, with each
+    pair's kernel in how: 'input_side', 'combined', 'tc' or 'simt').  U [pairs, E, 64]: radial coordinates of the low-rank pairs
+    lr = {pair: plan entry}; g [pairs, E, 128]: trunk outputs for the direct kernels.  Outputs go to outs {do: [E, Co, 2do+1]},
+    or on the production route to pooled or aligned_out."""
 
-    def __init__(self, conv, sw, route, U, g, lr, z, how, outs):
-        self.conv, self.sw, self.route, self.U, self.g, self.lr, self.z, self.how, self.outs = conv, sw, route, U, g, lr, z, how, outs
+    def __init__(self, d, U, g, how, outs):
+        self.d, self.U, self.g, self.how, self.outs = d, U, g, how, outs
         self.pooled = self.self_out = None
         self.aligned_out = {}
 
+    conv = property(operator.attrgetter('d.conv'))
+    sw = property(operator.attrgetter('d.sw'))
+    plan = property(operator.attrgetter('d.plan'))
+    route = property(operator.attrgetter('d.route'))
+    lr = property(operator.attrgetter('d.lr'))
 
-def _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing):
+
+def _forward_plan(conv, sw, tc_ok, E, rel_dist, geom):
     """The low-rank plan this forward of `conv` reads, or None (direct kernels)."""
     pk = conv.packed(sw)
     if sw.no_lowrank or conv.edge_dim != 0:
@@ -739,21 +756,21 @@ def _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing):
         return pk['lr']                     # built by pack_weights(max_distance=...) before the masters went away:
                                             # the only image there is, whatever the edge count
     if ops.lowrank_enabled(E, sw) and any(tc_ok.values()) and not conv.free_master and not conv._lr_blocked:
-        if capturing:
+        if torch.cuda.is_current_stream_capturing():
             return pk['lr']                 # built by the warm-up forwards; the residual check still covers it
         # cached; needs the distance range (one host sync per forward, in Geometry)
         return conv.lowrank_plan(geom.d_max(rel_dist) if geom is not None else float(rel_dist.max()), sw)
     return None
 
 
-def conv_decide(conv, E, rel_dist, geom, capturing):
-    """The per-forward half of conv_dispatch, from the whole graph (E edges, distances rel_dist): the switches, tc_ok and the
+def conv_decide(conv, E, rel_dist, geom):
+    """What `conv` decides once per forward, from the whole graph (E edges, distances rel_dist): the switches, tc_ok and the
     low-rank plan, which therefore stay the same in every node chunk.  A plan's run-time check is queued on geom.deferred
     here, once, over stats that the radial launches of all chunks accumulate into; without a deferred list conv_dispatch
     checks it after its launches."""
     sw = switches.current()
     tc_ok = {pair: conv.tc_eligible(*pair) for pair in conv.pairs}
-    plan = _forward_plan(conv, sw, tc_ok, E, rel_dist, geom, capturing)
+    plan = _forward_plan(conv, sw, tc_ok, E, rel_dist, geom)
     if plan is None or not plan['pairs']:
         return ConvDecision(conv, sw, tc_ok, None, None, False)
     stats = torch.zeros((len(conv.pairs), 2), dtype=torch.float32, device=rel_dist.device)
@@ -763,71 +780,73 @@ def conv_decide(conv, E, rel_dist, geom, capturing):
     return ConvDecision(conv, sw, tc_ok, plan, stats, deferred)
 
 
-def conv_dispatch(conv, edge_info, rel_dist, geom, capturing, decision=None):
-    """Launch the radial kernels of `conv` on these edges (U of the low-rank pairs from the plan's table or the trunk, g for the
-    direct kernels) under `decision` (conv_decide on these edges if None), and set up its outputs."""
-    idx = edge_info[0]
+def conv_dispatch(d, edge_info, rel_dist, geom):
+    """Launch the radial kernels of the convolution of decision d on these edges (U of the low-rank pairs from the plan's table
+    or the trunk, g for the direct kernels) and set up its outputs.  A plan miss checked here replaces d by the decision
+    without a plan."""
+    conv, idx = d.conv, edge_info[0]
     E, dev = idx.numel(), idx.device
-    d = conv_decide(conv, E, rel_dist, geom, capturing) if decision is None else decision
-    sw, tc_ok, plan = d.sw, d.tc_ok, d.plan
-    pk = conv.packed(sw)
+    pk = conv.packed(d.sw)
     feat = conv.edge_features(edge_info, rel_dist)
     assert feat.shape[-1] == conv.in_dim, f'edge feature width {feat.shape[-1]} != {conv.in_dim}'
-    lr, U, g, route = {}, None, None, 'rfirst'
+    U = g = None
+    plan = d.plan
     if plan is not None:
         covered = len(plan['pairs']) == len(conv.pairs)
-        stats = d.stats
-        if covered and plan['utab'] is not None and not sw.no_utable:
-            U = ops.radial_table(rel_dist, plan['utab'], plan['D'], plan['ones_col'], stats)
+        if covered and plan['utab'] is not None and not d.sw.no_utable:
+            U = ops.radial_table(rel_dist, plan['utab'], plan['D'], plan['ones_col'], d.stats)
         else:
-            U, g = ops.radial_trunk_u(feat, pk['trunk'], plan['Vstack'], plan['gmean'], plan['ones_col'], stats, want_g=not covered)
-        lr = dict(d.lr)
-        if not d.deferred and check_lowrank_stats([(conv, stats, plan['have'])]):
+            U, g = ops.radial_trunk_u(feat, pk['trunk'], plan['Vstack'], plan['gmean'], plan['ones_col'], d.stats, want_g=not covered)
+        if not d.deferred and check_lowrank_stats([(conv, d.stats, plan['have'])]):
             # the fp32 trunk outputs of this forward leave the cached subspace (distances beyond the plan's range)
             if conv.free_master:
                 raise LowRankPlanMiss('low-rank radial plan does not cover this input; pack_weights(max_distance=...) was given too '
                                       'small a distance')
-            lr = {}                              # evaluate this ConvSE3 with the direct K = 128 kernels
-    kinds = {pp['kind'] for pp in lr.values()}
-    if kinds & {'z', 'aligned'}:                 # edge-aligned plans cover every pair of the ConvSE3 and need the Geometry
-        if geom is None:
-            raise RuntimeError('ConvSE3 was called with a (flat, plan) basis: the edge-aligned low-rank plan needs the third element, '
-                               'model.Geometry(rel_pos, max_degree), as SE3Transformer.forward passes it (or set SE3B200_NO_ALIGNED=1)')
-        route = 'production' if 'z' in kinds else 'aligned'
-    elif len(lr) < len(conv.pairs) and g is None:
+            d = ConvDecision(conv, d.sw, d.tc_ok, None, None, False)       # evaluate this ConvSE3 with the direct K = 128 kernels
+    if d.route != 'rfirst' and geom is None:     # edge-aligned plans cover every pair of the ConvSE3 and need the Geometry
+        raise RuntimeError('ConvSE3 was called with a (flat, plan) basis: the edge-aligned low-rank plan needs the third element, '
+                           'model.Geometry(rel_pos, max_degree), as SE3Transformer.forward passes it (or set SE3B200_NO_ALIGNED=1)')
+    if d.direct and g is None:
         g = ops.radial_trunk(feat, pk['trunk'], len(conv.pairs))       # the direct kernels consume g itself
-    how = {pair: lr[pair]['kind'] if pair in lr else 'tc' if tc_ok[pair] else 'simt' for pair in conv.pairs}
+    how = {pair: d.lr[pair]['kind'] if pair in d.lr else 'tc' if d.tc_ok[pair] else 'simt' for pair in conv.pairs}
     # (the production route allocates the outputs it writes in _production_forward: pooled ones go to the nodes directly)
-    outs = {} if route == 'production' else \
+    outs = {} if d.route == 'production' else \
         {do: torch.empty((E, mo, to_order(do)), dtype=torch.float32, device=dev) for do, mo in conv.fiber_out}
-    return ConvDispatch(conv, sw, route, U, g, lr, plan['z'] if route == 'production' else None, how, outs)
+    return ConvDispatch(d, U, g, how, outs)
+
+
+def split_basis(basis):
+    """The basis argument of ConvSE3, AttentionSE3 and conv_forward -- (flat, BasisPlan), (flat, BasisPlan, Geometry) or
+    (None, None, Geometry) -- as (flat, BasisPlan, Geometry or None)."""
+    if isinstance(basis, dict):
+        raise TypeError("ConvSE3 takes the basis as the tuple (flat buffer, BasisPlan, Geometry) that SE3Transformer.forward builds: "
+                        "`ops.basis_flat(rel_pos, max_degree) + (model.Geometry(rel_pos, max_degree),)`; the dict returned by the "
+                        "drop-in get_basis() is the reference's per-pair view of the same buffer and is not accepted here")
+    flat, plan = basis[:2]
+    return flat, plan, basis[2] if len(basis) > 2 else None
 
 
 def conv_forward(convs, inp, edge_info, rel_dist, basis, keep_aligned=False, decisions=None, self_out=None, sx=None):
     """Evaluate one or more ConvSE3 that share input features, graph and fibers (to_k / to_v of an attention block)
     in a single sweep: the T blocks (gather x basis) are built once per (degree pair, edge chunk) and consumed by every
-    convolution's fused pairwise kernel.  conv_dispatch chooses each convolution's route; the production convolutions run
-    first, then the edge-aligned ones, then the R-first ones (the last two share one T workspace).
+    convolution's fused pairwise kernel.  Each convolution's decision (conv_decide, made here just before its dispatch if
+    decisions is None) gives its route; the production convolutions run first, then the edge-aligned ones, then the R-first
+    ones (the last two share one T workspace).
 
-    basis: (flat, BasisPlan, Geometry), or (None, None, Geometry) to build the flat basis from the Geometry only if an R-first
-    route needs it.  For one node chunk of a larger graph (NodeChunk), the caller passes the chunk's edges, the features as
-    NodeChunk.src gives them, the chunk's Geometry and the whole graph's decisions (conv_decide), plus the chunk's rows of the
-    whole graph's self-interaction (self_out, one pooled convolution) and edge scales (sx [b', n', k], production route)."""
+    basis: see split_basis; (None, None, Geometry) builds the flat basis from the Geometry only if an R-first route needs it.
+    For one node chunk of a larger graph (over_node_chunks), the caller passes the chunk's edges, the features as
+    NodeChunk.src gives them, the chunk's Geometry and the whole graph's decisions, plus the chunk's rows of the whole graph's
+    self-interaction (self_out, one pooled convolution) and edge scales (sx [b', n', k], production route)."""
     c0 = convs[0]
     forward_only_guard('ConvSE3', convs, list(inp.values()) + [rel_dist])
     idx = edge_info[0]
     E = idx.numel()
-    if isinstance(basis, dict):
-        raise TypeError("ConvSE3 takes the basis as the tuple (flat buffer, BasisPlan, Geometry) that SE3Transformer.forward builds: "
-                        "`ops.basis_flat(rel_pos, max_degree) + (model.Geometry(rel_pos, max_degree),)`; the dict returned by the "
-                        "drop-in get_basis() is the reference's per-pair view of the same buffer and is not accepted here")
-    flat, plan = basis[:2]                   # BasisFlat (+ Geometry)
-    geom = basis[2] if len(basis) > 2 else None
-    capturing = torch.cuda.is_current_stream_capturing()
+    flat, plan, geom = split_basis(basis)
     states = []
-    for conv, decision in zip(convs, decisions or [None] * len(convs)):
+    for i, conv in enumerate(convs):
         assert conv.pairs == c0.pairs and conv.in_dim == c0.in_dim
-        states.append(conv_dispatch(conv, edge_info, rel_dist, geom, capturing, decision))
+        d = decisions[i] if decisions else conv_decide(conv, E, rel_dist, geom)
+        states.append(conv_dispatch(d, edge_info, rel_dist, geom))
     if self_out is not None:
         assert len(states) == 1
         states[0].self_out = self_out
@@ -896,7 +915,8 @@ def _zgemm_degree(st, do, mo, X, sx, e0, ec):
     """out' [ec, 2do+1, Co] (edge frame, component major) of output degree do on edges e0 .. e0 + ec: one zgemm per |m|, whose
     K segments are the 16-column blocks of U of every input degree."""
     conv, P = st.conv, to_order(do)
-    full = all((do, m) in st.z for m in range(do + 1))
+    z = st.plan['z']
+    full = all((do, m) in z for m in range(do + 1))
     if do == 0 and st.pooled is None:
         Op = st.outs[0][e0:e0 + ec]                   # [ec, mo, 1] is [ec, 1, mo]
     elif do in st.aligned_out:
@@ -906,7 +926,7 @@ def _zgemm_degree(st, do, mo, X, sx, e0, ec):
     else:
         Op = (torch.empty if full else torch.zeros)((ec, P, mo), dtype=torch.float32, device=sx.device)
     for m in range(do + 1):
-        zp = st.z.get((do, m))
+        zp = z.get((do, m))
         if zp is None:
             continue
         segs, alg = [], 0
@@ -1096,7 +1116,7 @@ class AttentionSE3(nn.Module):
         forward_only_guard('AttentionSE3', [self], list(features.values()))
         idx = edge_info[0]
         queries = self.to_q(features)
-        geom = basis[2] if isinstance(basis, tuple) and len(basis) > 2 else None
+        flat, plan, geom = split_basis(basis)
         # rotate-back fused into the attention kernel
         fuse = geom is not None and not switches.current().no_attn_rotate and ops.attn_aligned_supported(self.dim_head)
         # node-level work over the whole graph: node keys (linear_proj_keys), self and global keys / values, rotary queries
@@ -1121,49 +1141,30 @@ class AttentionSE3(nn.Module):
             self_keys['0'] = apply_rotary_pos_emb(self_keys['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
             self_values['0'] = apply_rotary_pos_emb(self_values['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
         convs = [self.to_v] if self.linear_proj_keys or self.to_k is None else [self.to_k, self.to_v]
-        capturing = torch.cuda.is_current_stream_capturing()
-        decisions = [conv_decide(conv, idx.numel(), rel_dist, geom, capturing) for conv in convs]
-        b, n, k = idx.shape
-        chunks = [NodeChunk(0, b, 0, n, whole=True)]
-        if geom is not None:
-            ckv = self.to_v.fiber_out[0]
-            chunks = geom.node_chunks(decisions, idx.shape, keep_aligned=fuse,
-                                      attn_bytes=0 if k_emb is None else 4 * ckv * (4 + self.linear_proj_keys) + 4 * k_emb.shape[-1])
+        decisions = [conv_decide(conv, idx.numel(), rel_dist, geom) for conv in convs]
         kv = (node_keys, self_keys, self_values, global_keys, global_values)
-        if len(chunks) == 1:
-            outputs = self._attend(chunks[0], features, queries, kv, k_emb, edge_info, rel_dist, basis, geom, decisions, fuse, None)
-        else:
-            sx = chunk_edge_scale(decisions, features, idx)
-            outputs = {d: torch.empty_like(q) for d, q in queries.items()}
-            for c in chunks:
-                cgeom = geom.chunk(c)
-                res = self._attend(c, features, queries, kv, k_emb, edge_info, rel_dist, (None, None, cgeom), cgeom, decisions, fuse,
-                                   c.rows(sx))
-                for d, t in res.items():
-                    c.rows(outputs[d]).copy_(t)
+        attn_bytes = 0 if k_emb is None else 4 * self.to_v.fiber_out[0] * (4 + self.linear_proj_keys) + 4 * k_emb.shape[-1]
+        outputs = over_node_chunks((flat, plan, geom), decisions, features, idx,
+                                   lambda c, cbasis, sx: self._attend(c, features, queries, kv, k_emb, edge_info, rel_dist, cbasis,
+                                                                      decisions, fuse, sx),
+                                   keep_aligned=fuse, attn_bytes=attn_bytes)
         if isinstance(self.to_out, LinearSE3):
             return self.to_out(outputs, residual=residual)             # residual added in the epilogue of to_out
         return outputs if residual is None else residual_add(outputs, residual)
 
-    def _attend(self, c, features, queries, kv, k_emb, edge_info, rel_dist, basis, geom, decisions, fuse, sx):
-        """The edge work of node chunk c: keys / values of its edges (the convolutions under the whole graph's decisions), then
-        attention of its queries -> {degree: [b', n', H*Dh, 2d+1]}.  geom: the chunk's Geometry (basis[2]); sx: the chunk's rows
-        of the whole graph's edge scales (chunk_edge_scale), None for the whole graph."""
+    def _attend(self, c, features, queries, kv, k_emb, edge_info, rel_dist, basis, decisions, fuse, sx):
+        """The edge work of node chunk c (over_node_chunks): keys / values of its edges (the convolutions of the whole graph's
+        decisions, keys first), then attention of its queries -> {degree: [b', n', H*Dh, 2d+1]}.  basis: the chunk's; sx: its
+        rows of the whole graph's edge scales, None for the whole graph."""
         node_keys, self_keys, self_values, global_keys, global_values = kv
         edge_info = c.edge_info(edge_info)
         idx, nmask, _ = edge_info
-        src = c.src(features)
-        k_idx = None
+        _, _, geom = basis
+        outs = conv_forward([d.conv for d in decisions], c.src(features), edge_info, c.rows(rel_dist), basis, keep_aligned=fuse,
+                            decisions=decisions, sx=sx)
+        keys, values, k_idx = outs[0], outs[-1], None          # tie_key_values: one convolution, keys = values
         if self.linear_proj_keys:
-            values = conv_forward([self.to_v], src, edge_info, c.rows(rel_dist), basis, keep_aligned=fuse, decisions=decisions, sx=sx)[0]
-            keys = c.src(node_keys)               # node level; the attention kernel gathers through idx
-            k_idx = idx
-        elif self.to_k is None:
-            values = conv_forward([self.to_v], src, edge_info, c.rows(rel_dist), basis, keep_aligned=fuse, decisions=decisions, sx=sx)[0]
-            keys = values
-        else:
-            keys, values = conv_forward([self.to_k, self.to_v], src, edge_info, c.rows(rel_dist), basis, keep_aligned=fuse,
-                                        decisions=decisions, sx=sx)
+            keys, k_idx = c.src(node_keys), idx                 # node level; the attention kernel gathers through idx
         if k_emb is not None:
             b_, n_, kk = idx.shape
             Dh, hk = self.dim_head, (1 if self.one_headed else self.heads)
@@ -1719,11 +1720,9 @@ class SE3Transformer(nn.Module):
         """Everything after the graph (reference S:1240-1375): conv_in, pre-convs, attention blocks, conv_out, norm, linear_out
         and the output format.  reduce (or None) maps every output [b, n, ...] to what is returned (pooling, unbatching).
         Returns (output, the deferred run-time checks of the low-rank plans)."""
-        geom = Geometry(rel_pos, self.num_degrees - 1)
-        geom.deferred = []
-        # every ConvSE3 and attention block runs its edge work over node chunks under this budget (DESIGN.md 4.7); the flat
+        # every ConvSE3 and attention block runs its edge work over node chunks under the edge budget (DESIGN.md 4.7); the flat
         # basis is built by the Geometry of a chunk (or of the whole graph) only when an R-first convolution reads it
-        geom.edge_budget = edge_budget_bytes(switches.current(), rel_pos.device)
+        geom = Geometry(rel_pos, self.num_degrees - 1, deferred=[], edge_budget=edge_budget_bytes(switches.current(), rel_pos.device))
         basis = (None, None, geom)
         x = self.conv_in(feats, edge_info, rel_dist=rel_dist, basis=basis)
         for conv, nonlin in self.convs:
