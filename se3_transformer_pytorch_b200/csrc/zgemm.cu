@@ -29,7 +29,7 @@
 // the accumulator is added into the partial sums with round-to-nearest adds and restarted.  MODE 3 keeps both of its planes
 // in shared memory (per-thread float4 slots) and S1 in registers.  MODE 1 / 3 commit one wgmma group per K chunk and
 // generate the next chunk while the previous chunks' MMAs are in flight, with X loaded into registers a stage ahead; MODE 2 / 4
-// wait for their MMAs every stage.
+// wait for their MMAs every stage.  Every mode hands a stage's weight slot back to the producer at the end of that stage.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 #include <algorithm>
@@ -40,16 +40,16 @@ namespace se3 {
 
 constexpr int kZThreads = 384;
 constexpr int kZMaxSeg = 16;
-constexpr uint32_t kZWRingBytes = 196608;     // shared memory for the weight ring
 constexpr uint32_t kZSmemMax = 232448;        // dynamic shared memory of one CTA on sm_90
 
 // Shared memory of one CTA: 1 KiB alignment slack, the weight ring of WS stages, MODE 3's two planes (+m, -m) of fp32 partial
-// sums (64 floats per consumer thread each), the ring's mbarriers.  MODE 3 fills what is left after the planes with ring stages.
+// sums (64 floats per consumer thread each), the ring's mbarriers.  Every mode fills what is left with ring stages, up to 8:
+// MODE 1 / 4 7 stages of 32 KiB, MODE 2 8 of 16 KiB, MODE 3 3 of 32 KiB next to its planes.
 template <int MODE, int NC>
 struct ZSmem {
   static constexpr uint32_t kStageBytes = 2u * NC * 128u;                 // hi and lo rows of one stage
   static constexpr uint32_t kPlaneBytes = (MODE == 3) ? 2u * 256u * 64u * 4u : 0u;
-  static constexpr uint32_t kRingBytes = (MODE == 3) ? kZSmemMax - 1024u - 256u - kPlaneBytes : kZWRingBytes;
+  static constexpr uint32_t kRingBytes = kZSmemMax - 1024u - 256u - kPlaneBytes;
   static constexpr int WS = (kRingBytes / kStageBytes > 8) ? 8 : (int)(kRingBytes / kStageBytes);
   static constexpr size_t kBytes = 1024 + (size_t)WS * kStageBytes + kPlaneBytes + 256;
   static_assert(kBytes <= kZSmemMax, "shared memory");
@@ -234,16 +234,16 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
     fresh = (1 << NA) - 1;
     blk_start = s + 1;
   };
-  // MODE 2 / 4: the MMAs of stage s retire before the next stage is generated
+  // every MMA of stage s retires before the next stage is generated, and the stage's weight slot goes back to the producer
   auto finish_stage = [&](int s) {
-    wgmma_commit();
     wgmma_wait0();
     release(s);
     if (drain_after(s)) drain(s);
   };
 
   // MODE 1 / 3: one commit group per K chunk, so the MMAs of the last ZR - 1 chunks stay in flight while the next chunk's A
-  // fragments are generated
+  // fragments are generated.  The stage still ends with a full wait (ptxas would insert one at the loop back-edge, C7517), and
+  // its slot is returned right after it, so the producer stays WS - 1 stages ahead: MODE 3's 3-stage ring has no slot to spare.
   constexpr int ZR = 4;
   float u[2][4];                               // U[e, kq, kq+1, kq+8, kq+9] * sx[e] of rows r0, r0 + 8 (current segment)
   auto zf = [&](const float (&y)[2], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
@@ -254,25 +254,16 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
       for (int q = 0; q < 4; ++q) v[rs][q] = u[rs][q] * y[rs];
     z_frag(v, hi, lo);
   };
-  // chunk C of stage s into accumulator A.  The wait retires chunk k - ZR, whose A fragment registers the new chunk reuses; at
-  // C == ZR - 1 that is the last chunk of stage s - 1, so its weight slot goes back.
-  auto chunk_mma = [&](auto cc, auto ac, int s, const float (&y)[2], uint64_t b_hi, uint64_t b_lo) {
+  // chunk C of stage s into accumulator A.  The wait retires chunk k - ZR, whose A fragment registers the new chunk reuses.
+  auto chunk_mma = [&](auto cc, auto ac, const float (&y)[2], uint64_t b_hi, uint64_t b_lo) {
     constexpr int C = decltype(cc)::value, A = decltype(ac)::value;
     wgmma_wait<ZR - 1>();
-    if (C == ZR - 1 && s != blk_start) release(s - 1);     // stage s - 1 was not drained: its slot is still held
     uint32_t hi[4], lo[4];
     zf(y, hi, lo);
     wgmma_fence();
     z_mma3<NR>(D[A], hi, lo, b_hi + 2 * C, b_lo + 2 * C, ((fresh >> A) & 1) ^ 1);
     fresh &= ~(1 << A);
     wgmma_commit();
-  };
-  auto end_stage = [&](int s) {
-    if (drain_after(s)) {
-      wgmma_wait0();
-      release(s);
-      drain(s);
-    }
   };
   auto wait_stage = [&](int s, uint64_t& b_hi, uint64_t& b_lo) {
     mbar_wait(bar_w_full + 8 * (s % WS), (uint32_t)(s / WS) & 1u);
@@ -316,6 +307,7 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
       wgmma_fence();
 #pragma unroll
       for (int c = 0; c < 4; ++c) z_mma3<NR>(D[0], hi[c], lo[c], b_hi + 2 * c, b_lo + 2 * c);
+      wgmma_commit();
       finish_stage(s);
     }
 #pragma unroll
@@ -364,11 +356,11 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
           wait_stage(s, b_hi, b_lo);
           static_for<4>([&](auto cc) {
             constexpr int C = decltype(cc)::value;
-            chunk_mma(cc, ic<0>(), s, y[C], b_hi, b_lo);
+            chunk_mma(cc, ic<0>(), y[C], b_hi, b_lo);
 #pragma unroll
             for (int rs = 0; rs < 2; ++rs) y[C][rs] = __ldg(xn + C * istride + 8 * rs);
           });
-          end_stage(s);
+          finish_stage(s);
           xp = xn;
         }
       } else if constexpr (MODE == 2) {
@@ -407,6 +399,7 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
             z_mma3<NR>(D[NA - 1], hm[il], lm[il], ba_hi, ba_lo);
             z_mma3<NR>(D[NA - 1], hp[il], lp[il], bb_hi, bb_lo);
           }
+          wgmma_commit();
           finish_stage(s);
         }
       } else {
@@ -441,18 +434,18 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
             float y[2];
 #pragma unroll
             for (int rs = 0; rs < 2; ++rs) y[rs] = fmaf(fc, x[C][0][rs], fd * x[C][1][rs]);
-            chunk_mma(cc, ic<0>(), s, y, b_hi, b_lo);
+            chunk_mma(cc, ic<0>(), y, b_hi, b_lo);
 #pragma unroll
             for (int rs = 0; rs < 2; ++rs) {
               x[C][0][rs] = __ldg(xn + C * istride + 8 * rs);
               x[C][1][rs] = __ldg(xn + dmo + C * istride + 8 * rs);
             }
           });
+          wgmma_wait0();
+          release(s);
           if (set_end || s + 1 - blk_start == FS) {
             // S1 (set a+b) collects in registers; set a ends with -m += S1 + S2, set b with +m += S1 - S3 (a drain inside a set
             // adds +-D alone)
-            wgmma_wait0();
-            release(s);
             if (set == 0) {
 #pragma unroll
               for (int j = 0; j < NR; ++j) acc[0][j] = set_open ? acc[0][j] + D[0][j] : D[0][j];
