@@ -81,6 +81,15 @@ int se3_knn_fwd(const float* coors, const int64_t* cu_seqlens, const int* k_per_
                 float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist,
                 void* stream);
 
+/* The same search for the new rows of clouds that grow node by node (causal decoding): rows [row0, row0 + nrows) of each of b
+ * clouds, over the cloud's first n nodes.  coors [b, ld, 3] and node_mask [b, ld] (may be NULL) hold each cloud with a leading
+ * dimension of ld >= n nodes; neighbor_mask [b, nrows, n] uint8 (may be NULL) holds the new rows' masks.  Outputs [b, nrows, k]
+ * (rel_pos [b, nrows, k, 3]), indices local to the cloud, 1 <= k <= min(n - 1, 4096).  Each row is bit for bit the row that
+ * se3_knn_fwd writes for the same cloud of n nodes (uniform form, same k, dense masks). */
+int se3_knn_rows_fwd(const float* coors, const uint8_t* node_mask, const uint8_t* neighbor_mask, int b, int64_t n, int64_t ld,
+                     int row0, int nrows, int k, float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask,
+                     float* out_rel_pos, float* out_rel_dist, void* stream);
+
 /* Position of every neighbour in a sparse pair list (as in se3_pairs; batch_stride 0 when shared, else n): out[b,i,kk] = p with
  * cols[p] == idx[b,i,kk] inside row (b, i), or -1 if the row lacks that column.  idx, out: [b, n, k] int64.  The caller indexes
  * the list's values (edge tokens, edge features, hop counts) with a zero row appended for -1. */
@@ -226,6 +235,24 @@ int64_t se3_zgemm_image_bytes(int Co, int mode, int total_stages);
 int se3_zgemm_pack(const float* Fp, int Kp, int col0, int Co, int CiF, int mode, int total_stages, int stage0, void* image, void* stream);
 int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img, const float* sx, int64_t E, int Co, int mode,
                   float* out, int64_t out_edge_stride, int comp_off0, int comp_off1, int flush_stages, void* stream);
+
+/* Split-K of modes 1 and 3 for launches with few edge tiles: the stages of each output tile are shared by k_split CTAs, so that
+ * more of the card streams the weight image.  The fp32 partial sums of an output element are a fixed sequence of addends: one
+ * per drain block of flush_stages stages in mode 1, one per plane at each drain of weight sets a and b of every Gauss block in
+ * mode 3.  Each split takes a run of whole units (drain blocks / Gauss blocks) and writes every addend to its own slot of
+ * `workspace`; a second kernel adds the slots in their original order, starting from 0, and applies 1/sx.  The output is bit for
+ * bit that of se3_zgemm_fwd.  No float atomics: the result is deterministic.
+ *   se3_zgemm_split_units: the number of units of a launch, i.e. the largest k_split (1 for mode 2, which does not split; -1 for
+ *     bad arguments).  Mode 1 with flush_stages >= the stage count has one unit.
+ *   se3_zgemm_workspace_bytes: the workspace a split launch of E edges needs (0 for mode 2), whatever k_split:
+ *     [addend slots per plane][planes][E][Co] fp32, live edge rows only.
+ *   se3_zgemm_split_fwd: se3_zgemm_fwd's arguments, then k_split in [1, units] (1 runs se3_zgemm_fwd and reads no workspace), the
+ *     device workspace (16-byte aligned) and its size in bytes.  Mode 2 and mode 4 (LinearSE3) do not split. */
+int     se3_zgemm_split_units(const se3_zseg* segs, int n_seg, int Co, int mode, int flush_stages);
+int64_t se3_zgemm_workspace_bytes(const se3_zseg* segs, int n_seg, int64_t E, int Co, int mode, int flush_stages);
+int se3_zgemm_split_fwd(const se3_zseg* segs, int n_seg, const void* w_img, const float* sx, int64_t E, int Co, int mode,
+                        float* out, int64_t out_edge_stride, int comp_off0, int comp_off1, int flush_stages, int k_split,
+                        void* workspace, int64_t workspace_bytes, void* stream);
 
 /* Masked mean over the neighbour axis (utils.py:72-80): x [B, K, C] , mask [B, K] (NULL = plain mean) -> out [B, C]. */
 int se3_pool_fwd(const float* x, const uint8_t* mask, int64_t B, int K, int64_t C, float* out, void* stream);

@@ -246,6 +246,24 @@ knn_kernel(const float* __restrict__ coors, const int64_t* __restrict__ cu_seqle
                    out_rel_dist + o);
 }
 
+// One CTA per new row (cloud c, node i = row0 + r) of clouds that grow one step at a time: rows [row0, row0 + nrows) of b clouds
+// whose first n nodes are searched, stored with a leading dimension of ld >= n nodes (coors [b, ld, 3], node_mask [b, ld]);
+// nbr [b, nrows, n] holds the new rows' byte masks.  The row body is knn_row, so the results are those of knn_kernel's rows.
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS, 6)
+knn_rows_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mask, const uint8_t* __restrict__ nbr, int n,
+                int64_t ld, int row0, int nrows, int k, float valid_radius, int causal, int64_t* __restrict__ out_idx,
+                uint8_t* __restrict__ out_mask, float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
+  extern __shared__ unsigned long long keys[];
+  const int64_t t = blockIdx.x;
+  const int64_t c = t / nrows;
+  const int i = row0 + (int)(t % nrows);
+  const DensePairs pairs{nbr ? nbr + t * n : nullptr, nullptr};
+  const int64_t o = t * k;
+  knn_row<THREADS>(keys, coors + c * ld * 3, n, i, k, knn_npad(n), pairs, node_mask ? node_mask + c * ld : nullptr, valid_radius,
+                   causal, k, 0, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
+}
+
 __global__ void gather_pairs_kernel(const float* __restrict__ pf, const int64_t* __restrict__ idx, int n, int k, int e,
                                     int64_t total, float* __restrict__ out) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -355,6 +373,30 @@ extern "C" int se3_knn_fwd(const float* coors, const int64_t* cu_seqlens, const 
     return SE3_OK;
   };
   return csr ? launch(knn_kernel<THREADS, CsrPairs>) : launch(knn_kernel<THREADS, DensePairs>);
+}
+
+extern "C" int se3_knn_rows_fwd(const float* coors, const uint8_t* node_mask, const uint8_t* neighbor_mask, int b, int64_t n, int64_t ld,
+                                int row0, int nrows, int k, float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask,
+                                float* out_rel_pos, float* out_rel_dist, void* stream) {
+  using namespace se3;
+  SE3_REQUIRE(coors && out_idx && out_mask && out_rel_pos && out_rel_dist, "se3_knn_rows_fwd: null pointer");
+  SE3_REQUIRE(b > 0 && n > 1 && n < (1ll << 31) && ld >= n, "se3_knn_rows_fwd: need b > 0, 1 < n < 2^31, ld >= n (got b=%d n=%lld ld=%lld)",
+              b, (long long)n, (long long)ld);
+  SE3_REQUIRE(row0 >= 0 && nrows >= 1 && row0 + (int64_t)nrows <= n, "se3_knn_rows_fwd: rows [%d, %d + %d) outside the %lld nodes", row0,
+              row0, nrows, (long long)n);
+  SE3_REQUIRE(k >= 1 && k <= n - 1 && k <= KNN_TILE, "se3_knn_rows_fwd: k must be in [1, min(n-1, %d)] (got k=%d n=%lld)", KNN_TILE, k,
+              (long long)n);
+  SE3_REQUIRE((int64_t)b * nrows < (1ll << 31), "se3_knn_rows_fwd: %lld rows exceed the 1-D grid", (long long)b * nrows);
+  constexpr int THREADS = 256;
+  const int key_words = n - 1 > KNN_TILE ? KNN_TILE + next_pow2(k) : knn_npad((int)n);
+  const size_t smem = (size_t)key_words * sizeof(unsigned long long);
+  auto kernel = knn_rows_kernel<THREADS>;
+  if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)((int64_t)b * nrows), THREADS, smem, as_stream(stream)>>>(coors, node_mask, neighbor_mask, (int)n, ld, row0, nrows,
+                                                                              k, valid_radius, causal, out_idx, out_mask, out_rel_pos,
+                                                                              out_rel_dist);
+  SE3_LAUNCH_OK();
+  return SE3_OK;
 }
 
 extern "C" int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx,

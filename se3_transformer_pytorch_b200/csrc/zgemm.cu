@@ -91,7 +91,33 @@ struct ZParams {
   int64_t out_es;            // floats per edge row of out
   int comp_off[2];           // offset of the component plane(s) inside an edge row
   int n_mt, n_nt, S, flush_stages;
+  float* ws;                 // split-K: the addends [slots][planes][E][n_nt * N] (zsplit_layout), reduced by zsplit_reduce_kernel
+  int k_split, n_units;      // split-K: CTAs per output tile, split units (drain blocks / Gauss blocks) they share
 };
+
+// Split-K (SPLIT kernels).  The fp32 partial sums of an output element are ((0 + t1) + t2) + ... over a fixed sequence of
+// addends: MODE 1 adds one per drain block (flush_stages stages, the last one shorter), MODE 3 one per plane at every drain of
+// set a (-m) and of set b (+m), ceil(L / flush_stages) per set of each Gauss block.  Each addend depends only on the stages of
+// its own unit (drain block / Gauss block), and at a unit boundary the unsplit kernel holds nothing but its fp32 planes, so the
+// k_split CTAs of an output tile take consecutive ranges of whole units, store each addend in its own workspace slot, and a
+// reduction adds the slots in their original order: bit for bit what k_split = 1 writes.
+// Stage and first addend slot (per plane) of unit u, 0 <= u <= units (u = units: the end).
+__host__ __device__ inline void zunit_start(const ZSeg* seg, int n_seg, int mode, int FS, int S, int u, int& stage, int& slot) {
+  if (mode != 3) {
+    const int64_t st = (int64_t)u * FS;
+    stage = st < S ? (int)st : S;
+    slot = u;
+    return;
+  }
+  stage = slot = 0;
+  for (int i = 0; i < n_seg; ++i) {
+    const int L = zgauss_block(seg[i].Ci / 4), nb = seg[i].Ci / (4 * L), per = (L + FS - 1) / FS;
+    const int take = u < nb ? u : nb;
+    stage += 3 * L * take;
+    slot += per * take;
+    u -= take;
+  }
+}
 
 // MODE 3's planes of fp32 partial sums: 16-byte slots in shared memory, kept in program order (one slot live at a time)
 __device__ __forceinline__ float4 lds128(uint32_t a) {
@@ -125,10 +151,11 @@ __device__ __forceinline__ void z_mma3(float (&d)[NR], const uint32_t (&hi)[4], 
   }
 }
 
-template <int MODE, int N, int NC>
+template <int MODE, int N, int NC, bool SPLIT = false>
 __global__ void __launch_bounds__(kZThreads, 1)
 zgemm_kernel(const __grid_constant__ ZParams prm) {
   static_assert((MODE == 2) ? NC == 64 : NC == 128, "CTA width");
+  static_assert(!SPLIT || MODE == 1 || MODE == 3, "split-K runs modes 1 and 3");
   static_assert(N % NC == 0 && (MODE == 1 || N == 128), "weight image tile");
   constexpr int NA = (MODE == 2) ? 2 : 1;                      // accumulators
   constexpr int NO = (MODE == 2 || MODE == 3) ? 2 : 1;        // output planes
@@ -151,8 +178,20 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int S = prm.S, FS = prm.flush_stages;
   const int n_ct = prm.n_nt * NH;
-  const int ctile = (int)(blockIdx.x % n_ct);
-  const int64_t mt = blockIdx.x / n_ct;
+  unsigned tile = blockIdx.x;
+  // stages [sb, se) of this CTA, the first addend slot of each plane (SPLIT: split z of the tile's units, see zunit_start)
+  int sb = 0, se = S, slot0 = 0;
+  if constexpr (SPLIT) {
+    const unsigned tiles = (unsigned)prm.n_mt * (unsigned)n_ct;       // the grid has < 2^31 CTAs
+    const int z = (int)(blockIdx.x / tiles);
+    tile = blockIdx.x % tiles;
+    const int u0 = (int)((int64_t)z * prm.n_units / prm.k_split), u1 = (int)((int64_t)(z + 1) * prm.n_units / prm.k_split);
+    int unused;
+    zunit_start(prm.seg, prm.n_seg, MODE, FS, S, u0, sb, slot0);
+    zunit_start(prm.seg, prm.n_seg, MODE, FS, S, u1, se, unused);
+  }
+  const int ctile = (int)(tile % n_ct);
+  const int64_t mt = tile / n_ct;
   const int nt = ctile / NH, hs = ctile % NH;
 
   if (threadIdx.x == 0) {
@@ -172,9 +211,9 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
     if (warp == 0 && lane == 0) {
       // ===================== weight producer =====================
       const uint8_t* wsrc = prm.w_img + (size_t)nt * S * kImgStage + (size_t)hs * NC * 128u;
-      for (int s = 0; s < S; ++s) {
-        const int slot = s % WS;
-        mbar_wait(bar_w_empty + 8 * slot, ((uint32_t)(s / WS) & 1u) ^ 1u);
+      for (int s = sb; s < se; ++s) {
+        const int slot = (s - sb) % WS;
+        mbar_wait(bar_w_empty + 8 * slot, ((uint32_t)((s - sb) / WS) & 1u) ^ 1u);
         mbar_arrive_expect_tx(bar_w_full + 8 * slot, kStageBytes);
         bulk_g2s(sW + slot * kStageBytes, wsrc + (size_t)s * kImgStage, NC * 128u, bar_w_full + 8 * slot);
         bulk_g2s(sW + slot * kStageBytes + NC * 128u, wsrc + (size_t)s * kImgStage + N * 128u, NC * 128u, bar_w_full + 8 * slot);
@@ -208,28 +247,46 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
   // MODE 3's planes (+m at plane, -m at plane + 64 KiB): float4 slot g (fragment registers 4g .. 4g+3) of this thread at
   // (g * 256 + ct) * 16 B, conflict-free
   const uint32_t plane = sPlane + 16u * ct;
-  if constexpr (MODE == 3)
+  if constexpr (MODE == 3 && !SPLIT)
 #pragma unroll
     for (int g = 0; g < NR / 2; ++g) sts128(plane + 4096u * g, make_float4(0.f, 0.f, 0.f, 0.f));
-  int blk_start = 0;
+  int blk_start = sb;
+  // SPLIT: the next addend slot of plane +m (MODE 1: the only plane) and of plane -m
+  int slot_p = slot0, slot_m = slot0;
+  // SPLIT: addend t(j) of fragment register j into slot `slot` of plane `pl`, live rows only
+  auto store_addend = [&](int slot, int pl, auto&& t) {
+    const int Co = prm.n_nt * N;
+#pragma unroll
+    for (int rs = 0; rs < 2; ++rs) {
+      if (!live[rs]) continue;
+      float* dst = prm.ws + (((size_t)slot * NO + pl) * prm.E + eg[rs]) * Co + (size_t)ctile * NC + kq;
+#pragma unroll
+      for (int g = 0; g < NC / 8; ++g)
+        *reinterpret_cast<float2*>(dst + 8 * g) = make_float2(t(4 * g + 2 * rs), t(4 * g + 2 * rs + 1));
+    }
+  };
   // MODE 1 / 3 restart a drained accumulator with the first MMA that writes it (scale-d = 0) instead of zeroing its registers,
   // so D is written only by wgmma (bit a: accumulator a is drained).
   int fresh = 0;
 
   auto release = [&](int s) {                  // every MMA that read the weight slot of stage s has retired
     __syncwarp();
-    if (lane == 0) mbar_arrive(bar_w_empty + 8 * (s % WS));
+    if (lane == 0) mbar_arrive(bar_w_empty + 8 * ((s - sb) % WS));
   };
   // the accumulators are added into the fp32 partial sums at the end of each block of flush_stages stages, and after the last
-  auto drain_after = [&](int s) { return s + 1 == S || s + 1 - blk_start == FS; };
+  auto drain_after = [&](int s) { return s + 1 == se || s + 1 - blk_start == FS; };
   auto drain = [&](int s) {
+    if constexpr (SPLIT) {
+      store_addend(slot_p++, 0, [&](int j) { return D[0][j]; });
+    } else {
 #pragma unroll
-    for (int j = 0; j < NR; ++j) {
+      for (int j = 0; j < NR; ++j) {
 #pragma unroll
-      for (int a = 0; a < NA; ++a) acc[a][j] += D[a][j];
-      if (MODE == 2 || MODE == 4)
+        for (int a = 0; a < NA; ++a) acc[a][j] += D[a][j];
+        if (MODE == 2 || MODE == 4)
 #pragma unroll
-        for (int a = 0; a < NA; ++a) D[a][j] = 0.f;
+          for (int a = 0; a < NA; ++a) D[a][j] = 0.f;
+      }
     }
     fresh = (1 << NA) - 1;
     blk_start = s + 1;
@@ -266,8 +323,8 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
     wgmma_commit();
   };
   auto wait_stage = [&](int s, uint64_t& b_hi, uint64_t& b_lo) {
-    mbar_wait(bar_w_full + 8 * (s % WS), (uint32_t)(s / WS) & 1u);
-    const uint32_t wb = sW + (uint32_t)(s % WS) * kStageBytes;
+    mbar_wait(bar_w_full + 8 * ((s - sb) % WS), (uint32_t)((s - sb) / WS) & 1u);
+    const uint32_t wb = sW + (uint32_t)((s - sb) % WS) * kStageBytes;
     b_hi = wg_desc_sw128(wb);
     b_lo = wg_desc_sw128(wb + NC * 128u);
   };
@@ -333,6 +390,16 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
     for (int sg = 0; sg < prm.n_seg; ++sg) {
       const ZSeg& z = prm.seg[sg];
       const int ns = z.n_stage;
+      // SPLIT: stages [sl0, sl1) of the segment are this CTA's (whole units); the global index s skips the others
+      int sl0 = 0, sl1 = ns;
+      if constexpr (SPLIT) {
+        sl0 = min(max(sb - s, 0), ns);
+        sl1 = min(max(se - s, 0), ns);
+        if (sl0 >= sl1) {
+          s += ns;
+          continue;
+        }
+      }
       const size_t istride = (size_t)z.ncomp * 128;                     // floats between consecutive input channels of X
       const float* xp = z.X + ((size_t)mt * z.Ci * z.ncomp + z.cplus) * 128 + r0;
       const float* xm = z.X + ((size_t)mt * z.Ci * z.ncomp + z.cminus) * 128 + r0;
@@ -344,14 +411,18 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
       }
       if constexpr (MODE == 1) {
         // chunk c of stage sl = input channel 4 sl + c; its rows are loaded one stage ahead, as soon as the chunk is generated
+        if constexpr (SPLIT) {
+          s += sl0;
+          xp += 4 * sl0 * istride;
+        }
         float y[4][2];
 #pragma unroll
         for (int c = 0; c < 4; ++c)
 #pragma unroll
           for (int rs = 0; rs < 2; ++rs) y[c][rs] = __ldg(xp + c * istride + 8 * rs);
 #pragma unroll 1
-        for (int sl = 0; sl < ns; ++sl, ++s) {
-          const float* xn = (sl + 1 < ns) ? xp + 4 * istride : xp;    // the last stage reloads its own rows, never past the tile
+        for (int sl = sl0; sl < sl1; ++sl, ++s) {
+          const float* xn = (sl + 1 < sl1) ? xp + 4 * istride : xp;   // the last stage reloads its own rows, never past the tile
           uint64_t b_hi, b_lo;
           wait_stage(s, b_hi, b_lo);
           static_for<4>([&](auto cc) {
@@ -363,6 +434,7 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
           finish_stage(s);
           xp = xn;
         }
+        if constexpr (SPLIT) s += ns - sl1;
       } else if constexpr (MODE == 2) {
 #pragma unroll 1
         for (int sl = 0; sl < ns; ++sl, ++s) {
@@ -410,6 +482,12 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
         const int L = zgauss_block(z.Ci / 4);
         const int dmo = (z.cminus - z.cplus) * 128;                   // from x'(+m) to x'(-m) of the same channel
         const int step = 4 * z.ncomp * 128, rewind = -(L - 1) * step; // to the next 4 channels, back to the set's first 4
+        int s_end = s + ns;
+        if constexpr (SPLIT) {                 // sl0 starts a Gauss block: 3 L stages per 4 L channels
+          s_end = s + sl1;
+          s += sl0;
+          xp += (sl0 / 3) * step;
+        }
         float x[4][2][2];                      // [chunk][c = x'(+m), d = x'(-m)][row]
 #pragma unroll
         for (int c = 0; c < 4; ++c)
@@ -420,7 +498,6 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
           }
         int left = L - 1, set = 0;             // stages left in the set after this one, set of the block
         bool set_open = false;                 // the current set has been drained before (S1 holds part of set a+b)
-        const int s_end = s + ns;
 #pragma unroll 1
         for (; s < s_end; ++s) {
           const bool set_end = left == 0;
@@ -449,6 +526,12 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
             if (set == 0) {
 #pragma unroll
               for (int j = 0; j < NR; ++j) acc[0][j] = set_open ? acc[0][j] + D[0][j] : D[0][j];
+            } else if constexpr (SPLIT) {
+              const bool sa = set == 1;
+              store_addend(sa ? slot_m++ : slot_p++, sa ? 1 : 0, [&](int j) {
+                const float d = D[0][j], s1 = acc[0][j];
+                return set_end ? (sa ? s1 + d : s1 - d) : (sa ? d : -d);
+              });
             } else {
               const uint32_t pl = plane + (set == 1 ? 65536u : 0u);
 #pragma unroll
@@ -479,13 +562,14 @@ zgemm_kernel(const __grid_constant__ ZParams prm) {
             --left;
           }
         }
+        if constexpr (SPLIT) s += ns - sl1;
       }
     }
 
-    // out'[e, component plane, channels of this CTA]
+    // out'[e, component plane, channels of this CTA] (SPLIT: written by zsplit_reduce_kernel)
 #pragma unroll
     for (int rs = 0; rs < 2; ++rs) {
-      if (!live[rs]) continue;
+      if (SPLIT || !live[rs]) continue;
       const float inv = 1.f / sxe[rs];
 #pragma unroll
       for (int a = 0; a < NO; ++a) {
@@ -538,12 +622,39 @@ __global__ void zpack_kernel(const float* __restrict__ Fp, int Kp, int col0, int
   }
 }
 
-template <int MODE, int N, int NC>
+// out'[e, plane p, c] = (sum of the workspace slots of (p, e, c) in slot order, from 0) / sx[e]: the epilogue of a split launch
+__global__ void zsplit_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ sx, int64_t E, int Co, int planes, int slots,
+                                     float* __restrict__ out, int64_t out_es, int off0, int off1) {
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= E * planes * Co) return;
+  const int c = (int)(t % Co), p = (int)(t / Co % planes);
+  const int64_t e = t / ((int64_t)Co * planes);
+  const size_t stride = (size_t)planes * E * Co;
+  const float* w = ws + ((size_t)p * E + e) * Co + c;
+  float r = 0.f;
+  for (int a = 0; a < slots; ++a) r += w[a * stride];
+  const float inv = 1.f / sx[e];
+  out[e * out_es + (p ? off1 : off0) + c] = r * inv;
+}
+
+// (split units, addend slots per plane) of a launch: the largest k_split and the workspace depth (zunit_start)
+static void zsplit_layout(const ZParams& prm, int mode, int& units, int& slots) {
+  if (mode == 1) {
+    units = slots = (int)ceil_div(prm.S, prm.flush_stages);
+    return;
+  }
+  units = 0;
+  for (int i = 0; i < prm.n_seg; ++i) units += prm.seg[i].Ci / (4 * zgauss_block(prm.seg[i].Ci / 4));
+  int stage;
+  zunit_start(prm.seg, prm.n_seg, mode, prm.flush_stages, prm.S, units, stage, slots);
+}
+
+template <int MODE, int N, int NC, bool SPLIT = false>
 static int launch_z(const ZParams& prm, cudaStream_t s) {
   const size_t smem = ZSmem<MODE, NC>::kBytes;
-  auto kern = zgemm_kernel<MODE, N, NC>;
+  auto kern = zgemm_kernel<MODE, N, NC, SPLIT>;
   SE3_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int64_t grid = (int64_t)prm.n_mt * prm.n_nt * (N / NC);
+  const int64_t grid = (int64_t)prm.n_mt * prm.n_nt * (N / NC) * (SPLIT ? prm.k_split : 1);
   SE3_REQUIRE(grid < 2147483647ll, "se3_zgemm: grid too large");
   kern<<<(unsigned)grid, kZThreads, smem, s>>>(prm);
   SE3_LAUNCH_OK();
@@ -614,16 +725,17 @@ extern "C" int se3_linear_tc_fwd(const float* x, const void* w_img, const float*
   return launch_z<4, 128, 128>(prm, as_stream(stream));
 }
 
-extern "C" int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img, const float* sx, int64_t E, int Co, int mode,
-                             float* out, int64_t out_edge_stride, int comp_off0, int comp_off1, int flush_stages, void* stream) {
-  using namespace se3;
+namespace se3 {
+
+// The launch parameters of se3_zgemm_fwd / se3_zgemm_split_fwd (everything but the split), checked.
+static int zgemm_params(const se3_zseg* segs, int n_seg, const void* w_img, const float* sx, int64_t E, int Co, int mode, float* out,
+                        int64_t out_edge_stride, int comp_off0, int comp_off1, int flush_stages, ZParams& prm) {
   const int N = se3_zgemm_tile_n(Co, mode);
   SE3_REQUIRE(N > 0 && mode != 4, "se3_zgemm_fwd: Co=%d must be a multiple of 128 and mode 1, 2 or 3 (got %d)", Co, mode);
   SE3_REQUIRE(E > 0 && n_seg >= 1 && n_seg <= kZMaxSeg, "se3_zgemm_fwd: bad sizes (1..%d segments)", kZMaxSeg);
   SE3_REQUIRE(segs != nullptr && w_img != nullptr && sx != nullptr && out != nullptr, "se3_zgemm_fwd: null pointer");
   SE3_REQUIRE(out_edge_stride >= Co && out_edge_stride % 4 == 0 && comp_off0 % 4 == 0 && comp_off1 % 4 == 0 &&
               (reinterpret_cast<uintptr_t>(out) & 15) == 0, "se3_zgemm_fwd: output rows must be 16-byte aligned");
-  ZParams prm;
   prm.n_seg = n_seg;
   int S = 0;
   const int F = (mode == 1) ? 1 : 2;          // MODE 1: one weight per (o,i); MODE 2 / 3: the pair (a, b)
@@ -655,8 +767,77 @@ extern "C" int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img,
   // default drain period: 96 accumulating K = 16 MMAs per accumulator (8 stages of 12; mode 3 also drains at the end of every
   // weight set, at most 8 stages): rel. error 4e-6 against float64 for all-positive operands at K = 65536 (2.5e-4 if never drained)
   prm.flush_stages = flush_stages > 0 ? flush_stages : 8;
+  prm.ws = nullptr;
+  prm.k_split = 1;
+  prm.n_units = 1;
+  return SE3_OK;
+}
+
+}  // namespace se3
+
+extern "C" int se3_zgemm_fwd(const se3_zseg* segs, int n_seg, const void* w_img, const float* sx, int64_t E, int Co, int mode,
+                             float* out, int64_t out_edge_stride, int comp_off0, int comp_off1, int flush_stages, void* stream) {
+  using namespace se3;
+  ZParams prm;
+  const int rc = zgemm_params(segs, n_seg, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off0, comp_off1, flush_stages, prm);
+  if (rc != SE3_OK) return rc;
+  const int N = se3_zgemm_tile_n(Co, mode);
   cudaStream_t s = as_stream(stream);
   if (mode == 3) return launch_z<3, 128, 128>(prm, s);
   if (mode == 2) return launch_z<2, 128, 64>(prm, s);
   return N == 256 ? launch_z<1, 256, 128>(prm, s) : launch_z<1, 128, 128>(prm, s);
+}
+
+extern "C" int se3_zgemm_split_units(const se3_zseg* segs, int n_seg, int Co, int mode, int flush_stages) {
+  using namespace se3;
+  if (mode != 1 && mode != 3) return (mode == 2) ? 1 : -1;
+  ZParams prm;
+  float dummy;
+  if (zgemm_params(segs, n_seg, &dummy, &dummy, 1, Co, mode, reinterpret_cast<float*>(16), Co, 0, 0, flush_stages, prm) != SE3_OK) return -1;
+  int units, slots;
+  zsplit_layout(prm, mode, units, slots);
+  return units;
+}
+
+extern "C" int64_t se3_zgemm_workspace_bytes(const se3_zseg* segs, int n_seg, int64_t E, int Co, int mode, int flush_stages) {
+  using namespace se3;
+  if (mode != 1 && mode != 3) return (mode == 2) ? 0 : -1;
+  ZParams prm;
+  float dummy;
+  if (E <= 0 || zgemm_params(segs, n_seg, &dummy, &dummy, E, Co, mode, reinterpret_cast<float*>(16), Co, 0, 0, flush_stages, prm) != SE3_OK) return -1;
+  int units, slots;
+  zsplit_layout(prm, mode, units, slots);
+  return (int64_t)slots * (mode == 3 ? 2 : 1) * E * Co * (int64_t)sizeof(float);
+}
+
+extern "C" int se3_zgemm_split_fwd(const se3_zseg* segs, int n_seg, const void* w_img, const float* sx, int64_t E, int Co, int mode,
+                                   float* out, int64_t out_edge_stride, int comp_off0, int comp_off1, int flush_stages, int k_split,
+                                   void* workspace, int64_t workspace_bytes, void* stream) {
+  using namespace se3;
+  if (k_split == 1)
+    return se3_zgemm_fwd(segs, n_seg, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off0, comp_off1, flush_stages, stream);
+  SE3_REQUIRE(mode == 1 || mode == 3, "se3_zgemm_split_fwd: modes 1 and 3 split (got mode %d with k_split %d)", mode, k_split);
+  ZParams prm;
+  const int rc = zgemm_params(segs, n_seg, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off0, comp_off1, flush_stages, prm);
+  if (rc != SE3_OK) return rc;
+  int units, slots;
+  zsplit_layout(prm, mode, units, slots);
+  SE3_REQUIRE(k_split >= 1 && k_split <= units, "se3_zgemm_split_fwd: k_split = %d outside [1, %d] (the launch's split units)", k_split, units);
+  const int planes = (mode == 3) ? 2 : 1;
+  const int64_t need = (int64_t)slots * planes * E * Co * (int64_t)sizeof(float);
+  SE3_REQUIRE(workspace != nullptr && (reinterpret_cast<uintptr_t>(workspace) & 15) == 0 && workspace_bytes >= need,
+              "se3_zgemm_split_fwd: the workspace needs %lld bytes, 16-byte aligned (got %lld)", (long long)need, (long long)workspace_bytes);
+  prm.ws = reinterpret_cast<float*>(workspace);
+  prm.k_split = k_split;
+  prm.n_units = units;
+  cudaStream_t s = as_stream(stream);
+  const int N = se3_zgemm_tile_n(Co, mode);
+  const int lrc = (mode == 3) ? launch_z<3, 128, 128, true>(prm, s)
+                  : (N == 256) ? launch_z<1, 256, 128, true>(prm, s) : launch_z<1, 128, 128, true>(prm, s);
+  if (lrc != SE3_OK) return lrc;
+  const int64_t total = E * planes * Co;
+  zsplit_reduce_kernel<<<(unsigned)ceil_div(total, 256), 256, 0, s>>>(prm.ws, sx, E, Co, planes, slots, out, out_edge_stride,
+                                                                     comp_off0, comp_off1);
+  SE3_LAUNCH_OK();
+  return SE3_OK;
 }

@@ -1115,12 +1115,36 @@ class AttentionSE3(nn.Module):
     def forward(self, features, edge_info, rel_dist, basis, global_feats=None, pos_emb=None, mask=None, residual=None):
         forward_only_guard('AttentionSE3', [self], list(features.values()))
         idx = edge_info[0]
-        queries = self.to_q(features)
         flat, plan, geom = split_basis(basis)
-        # rotate-back fused into the attention kernel
-        fuse = geom is not None and not switches.current().no_attn_rotate and ops.attn_aligned_supported(self.dim_head)
-        # node-level work over the whole graph: node keys (linear_proj_keys), self and global keys / values, rotary queries
-        node_keys = self.to_k(features) if self.linear_proj_keys else None
+        fuse = self.fuse_rotation(geom)
+        queries, kv, k_emb = self.node_level(features, global_feats, pos_emb)
+        decisions = [conv_decide(conv, idx.numel(), rel_dist, geom) for conv in self.edge_convs()]
+        attn_bytes = 0 if k_emb is None else 4 * self.to_v.fiber_out[0] * (4 + self.linear_proj_keys) + 4 * k_emb.shape[-1]
+        outputs = over_node_chunks((flat, plan, geom), decisions, features, idx,
+                                   lambda c, cbasis, sx: self._attend(c, features, queries, kv, k_emb, edge_info, rel_dist, cbasis,
+                                                                      decisions, fuse, sx),
+                                   keep_aligned=fuse, attn_bytes=attn_bytes)
+        return self.project_out(outputs, residual)
+
+    def fuse_rotation(self, geom):
+        """The rotate-back of the values is fused into the attention kernel."""
+        return geom is not None and not switches.current().no_attn_rotate and ops.attn_aligned_supported(self.dim_head)
+
+    def edge_convs(self):
+        """The convolutions that make keys and values on the edges, keys first."""
+        return [self.to_v] if self.linear_proj_keys or self.to_k is None else [self.to_k, self.to_v]
+
+    def project_out(self, outputs, residual):
+        if isinstance(self.to_out, LinearSE3):
+            return self.to_out(outputs, residual=residual)             # residual added in the epilogue of to_out
+        return outputs if residual is None else residual_add(outputs, residual)
+
+    def node_level(self, features, global_feats, pos_emb, node_keys=None):
+        """Node-level work of the nodes of `features`: queries, (node keys, self keys, self values, global keys, global values)
+        and the key rotary embedding; node_keys (linear_proj_keys) default to to_k of the features."""
+        queries = self.to_q(features)
+        if self.linear_proj_keys and node_keys is None:
+            node_keys = self.to_k(features)
         self_keys = self_values = global_keys = global_values = None
         if self.attend_self:
             self_keys, self_values = self.to_self_k(features), self.to_self_v(features)
@@ -1140,17 +1164,7 @@ class AttentionSE3(nn.Module):
             self_keys, self_values = dict(self_keys), dict(self_values)
             self_keys['0'] = apply_rotary_pos_emb(self_keys['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
             self_values['0'] = apply_rotary_pos_emb(self_values['0'].view(b_, n_, hk, Dh, 1), self_emb).reshape(b_, n_, -1, 1)
-        convs = [self.to_v] if self.linear_proj_keys or self.to_k is None else [self.to_k, self.to_v]
-        decisions = [conv_decide(conv, idx.numel(), rel_dist, geom) for conv in convs]
-        kv = (node_keys, self_keys, self_values, global_keys, global_values)
-        attn_bytes = 0 if k_emb is None else 4 * self.to_v.fiber_out[0] * (4 + self.linear_proj_keys) + 4 * k_emb.shape[-1]
-        outputs = over_node_chunks((flat, plan, geom), decisions, features, idx,
-                                   lambda c, cbasis, sx: self._attend(c, features, queries, kv, k_emb, edge_info, rel_dist, cbasis,
-                                                                      decisions, fuse, sx),
-                                   keep_aligned=fuse, attn_bytes=attn_bytes)
-        if isinstance(self.to_out, LinearSE3):
-            return self.to_out(outputs, residual=residual)             # residual added in the epilogue of to_out
-        return outputs if residual is None else residual_add(outputs, residual)
+        return queries, (node_keys, self_keys, self_values, global_keys, global_values), k_emb
 
     def _attend(self, c, features, queries, kv, k_emb, edge_info, rel_dist, basis, decisions, fuse, sx):
         """The edge work of node chunk c (over_node_chunks): keys / values of its edges (the convolutions of the whole graph's
@@ -1373,6 +1387,11 @@ class SE3Transformer(nn.Module):
             raise ValueError('graphed: sparse pair inputs are not supported (their number of entries is not static); pass dense '
                              'tensors or call forward')
         return GraphedForward(self, feats, coors, mask, **fwd_kwargs)
+
+    def causal_decoder(self, batch_size=1):
+        """An empty CausalDecoder of this causal model for batch_size clouds: generation one node (or a few) at a time, each step
+        doing the edge work of its new nodes only."""
+        return CausalDecoder(self, batch_size)
 
     # ---- forward ----------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -1731,6 +1750,10 @@ class SE3Transformer(nn.Module):
         x = self.net(x, edge_info=edge_info, rel_dist=rel_dist, basis=basis, global_feats=global_feats, pos_emb=pos_emb, mask=mask)
         if exists(self.conv_out):
             x = self.conv_out(x, edge_info, rel_dist=rel_dist, basis=basis)
+        return self._output(x, reduce, out_dtype, return_type), geom.deferred
+
+    def _output(self, x, reduce, out_dtype, return_type):
+        """The output format after conv_out: norm, linear_out, reduce (or None), type-0 squeeze, dtype and return_type."""
         x = self.norm(x)
         if exists(self.linear_out):
             x = self.linear_out(x)
@@ -1742,8 +1765,8 @@ class SE3Transformer(nn.Module):
         if exists(out_dtype):
             x = {k: v.to(out_dtype) for k, v in x.items()}
         if exists(return_type):
-            return x[str(return_type)], geom.deferred
-        return x, geom.deferred
+            return x[str(return_type)]
+        return x
 
     # ---- packed batches ------------------------------------------------------------------------------------
     def _check_packed(self, feats, coors, seqlens, adj_mat, edges, neighbor_mask):
@@ -1898,3 +1921,233 @@ class GraphedForward:
             raise LowRankPlanMiss('captured forward: the low-rank radial plan does not cover this input (distances beyond the range '
                                   'seen when the graph was captured); build a new graph or pack_weights(max_distance=...) for a larger range')
         return self.out
+
+
+FLT_MAX = 3.4028234663852886e38
+
+
+class _StepRows:
+    """The node chunk of a CausalDecoder step, in the batch-1 view with global indices that forward_packed uses: its rows are
+    the step's new nodes (row-level tensors are passed as they are) and its neighbours are gathered from the decoder's cache,
+    a [1, b * capacity, ...] tensor of which src() gives the view the kernels expect (NodeChunk.src)."""
+    b0, b1, whole = 0, 1, False
+
+    def __init__(self, rows):
+        self.n_rows = rows
+
+    def rows(self, t):
+        return t
+
+    def edge_info(self, edge_info):
+        return edge_info
+
+    def src(self, t):
+        if isinstance(t, dict):
+            return {key: self.src(v) for key, v in t.items()}
+        return t[:, :self.n_rows]
+
+
+class CausalDecoder:
+    """Generation with a causal SE3Transformer, node by node (SE3Transformer.causal_decoder).
+
+    Node i of a causal model depends only on nodes j <= i: the neighbour search gives every later column the key FLT_MAX, so
+    later nodes only fill masked slots, which get zero weight in the attention softmax and in the pooled means; everything else
+    is per node.  The decoder therefore keeps, per cloud and per stage, the node features that later nodes gather as neighbours
+    (the embedded input of conv_in, the input of each pre-convolution, prenorm(x) of every attention block and its node keys
+    with linear_proj_keys, the input of conv_out), with their node maxima (the production route's edge scales), in storage that
+    grows geometrically.  extend() searches the neighbours of the new rows only, runs every convolution and attention block over
+    the new nodes' edges and the node-level work over the new rows, and appends the new rows to the cache.
+
+    extend(feats, coors, ...) returns rows [n_prev, n_cur) of what forward returns for all nodes so far, with the [b, n, n] pair
+    inputs stacked from the rows given (anything above the diagonal).  The first call (the prefill) needs at least 2 nodes, as a
+    forward does.  Lockstep batches: every call adds the same number of nodes to each of the batch_size clouds."""
+
+    def __init__(self, model, batch_size=1):
+        if not model.causal:
+            raise ValueError('causal_decoder: the model is not causal (causal=False): the outputs of earlier nodes would change as '
+                             'nodes arrive, so they cannot be cached')
+        if model.attend_sparse_neighbors or exists(model.num_adj_degrees):
+            raise NotImplementedError('causal_decoder: attend_sparse_neighbors and num_adj_degrees are not supported: the number of '
+                                      'bonded neighbours and the hop counts depend on the whole adjacency, including future rows')
+        if model.accept_global_feats:
+            raise NotImplementedError('causal_decoder: models built with global_feats_dim are not supported (the attention kernel '
+                                      'indexes the global keys by batch row, and a decoding step is one row)')
+        if not model.valid_radius < FLT_MAX:
+            raise ValueError(f'causal_decoder: valid_radius = {model.valid_radius} >= FLT_MAX: the FLT_MAX keys of later nodes would '
+                             'count as valid neighbours, so even forward() is not causal; give a finite radius below FLT_MAX')
+        if operator.index(batch_size) < 1:
+            raise ValueError(f'causal_decoder: batch_size must be >= 1, got {batch_size}')
+        self.model, self.b = model, int(batch_size)
+        self.n = self.cap = 0
+        self.coors = self.mask = None             # [b, cap, 3] fp32, [b, cap] bool
+        self.stages = {}                          # name -> (feats {d: [b, cap, C, 2d+1]}, nodemax [b, cap])
+
+    def __len__(self):
+        return self.n
+
+    def cache_bytes_per_node(self):
+        """Bytes the cache holds per node of a cloud (features, node maxima, coordinates and mask)."""
+        per = 13
+        for feats, nodemax in self.stages.values():
+            per += sum(t[0, 0].numel() * 4 for t in feats.values()) + 4
+        return per
+
+    # ---- checks --------------------------------------------------------------------------------------------
+    def _check(self, feats, coors, mask, edges, neighbor_mask, return_pooled):
+        """Everything extend takes from the caller, checked before any device work; returns m."""
+        model, b = self.model, self.b
+        if return_pooled:
+            raise ValueError('extend: return_pooled is not supported: the mean over nodes changes with every node that arrives')
+        for name, t in (('edges', edges), ('neighbor_mask', neighbor_mask), ('mask', mask), ('coors', coors)):
+            if _is_sparse(t):
+                raise ValueError(f'extend: {name} is a sparse tensor; decoding takes dense rows (sparse pair inputs are not supported)')
+        if not torch.is_tensor(coors) or coors.dim() != 3 or coors.shape[0] != b or coors.shape[2] != 3 or coors.shape[1] < 1:
+            raise ValueError(f'extend: coors must be [batch_size, m, 3] with batch_size = {b}, m >= 1, got '
+                             f'{tuple(coors.shape) if torch.is_tensor(coors) else type(coors).__name__}')
+        m = coors.shape[1]
+        n_cur = self.n + m
+        if n_cur < 2:
+            raise ValueError('extend: the first call (the prefill) needs at least 2 nodes per cloud, as a forward does')
+        for t in (feats.values() if isinstance(feats, dict) else [feats]):
+            if not torch.is_tensor(t) or t.dim() < 2 or tuple(t.shape[:2]) != (b, m):
+                raise ValueError(f'extend: the features must be [batch_size, m, ...] = {(b, m)} like coors, got '
+                                 f'{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}')
+            if _is_sparse(t):
+                raise ValueError('extend: sparse features are not supported')
+        if mask is not None and (not torch.is_tensor(mask) or tuple(mask.shape) != (b, m)):
+            raise ValueError(f'extend: mask must be [batch_size, m] = {(b, m)}, got {tuple(mask.shape) if torch.is_tensor(mask) else type(mask).__name__}')
+        if neighbor_mask is not None and (not torch.is_tensor(neighbor_mask) or tuple(neighbor_mask.shape) != (b, m, n_cur)):
+            raise ValueError(f'extend: neighbor_mask must be the new rows [batch_size, m, n_cur] = {(b, m, n_cur)}, got '
+                             f'{tuple(neighbor_mask.shape) if torch.is_tensor(neighbor_mask) else type(neighbor_mask).__name__}')
+        if model.has_edges and edges is None:
+            raise ValueError('extend: the model has edge features (edge_dim): pass edges for the new rows')
+        if edges is not None:
+            if not model.has_edges:
+                raise ValueError('extend: edges given, but the model was built without edge_dim')
+            dims = 3 if exists(model.edge_emb) else 4
+            if not torch.is_tensor(edges) or edges.dim() != dims or tuple(edges.shape[:3]) != (b, m, n_cur):
+                shape = '[batch_size, m, n_cur]' if exists(model.edge_emb) else '[batch_size, m, n_cur, edge_dim]'
+                raise ValueError(f'extend: edges must hold the pair values of every new node to every node so far, {shape} with '
+                                 f'batch_size, m, n_cur = {(b, m, n_cur)}, got {tuple(edges.shape) if torch.is_tensor(edges) else type(edges).__name__}')
+        if exists(model.pos_emb) and n_cur > model.num_positions:
+            raise ValueError(f'extend: node {n_cur - 1} is past num_positions = {model.num_positions}')
+        return m
+
+    # ---- one step ------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def extend(self, feats, coors, mask=None, edges=None, neighbor_mask=None, return_type=None, return_pooled=False):
+        """Append m >= 1 nodes to each cloud and return their outputs, shaped like forward's for [batch_size, m] nodes.
+        feats [b, m, dim_in] float, [b, m] tokens or {'d': [b, m, C, 2d+1]}; coors [b, m, 3]; mask [b, m]; edges [b, m, n_cur]
+        tokens or [b, m, n_cur, edge_dim]; neighbor_mask [b, m, n_cur] (n_cur = len(self) + m)."""
+        m = self._check(feats, coors, mask, edges, neighbor_mask, return_pooled)
+        out = self.model._checked(lambda: self._step(feats, coors, mask, edges, neighbor_mask, return_type, m))
+        self.n += m
+        return out
+
+    def _grow(self, n_cur, dev):
+        """Capacity for n_cur nodes per cloud: doubled when full, so a step never copies the whole prefix."""
+        if n_cur <= self.cap:
+            return
+        cap = max(n_cur, 2 * self.cap, 16)
+
+        def grown(t):
+            new = t.new_empty((self.b, cap) + tuple(t.shape[2:]))
+            new[:, :self.n] = t[:, :self.n]
+            return new
+        if self.coors is None:
+            self.coors = torch.empty((self.b, 0, 3), dtype=torch.float32, device=dev)
+            self.mask = torch.ones((self.b, 0), dtype=torch.bool, device=dev)
+        self.coors, self.mask = grown(self.coors), grown(self.mask)
+        self.stages = {name: ({d: grown(t) for d, t in feats.items()}, grown(nodemax)) for name, (feats, nodemax) in self.stages.items()}
+        self.cap = cap
+
+    def _append(self, name, x, n0, m):
+        """Store the new rows x {d: [1, b m, C, 2d+1]} of stage `name` at [n0, n0 + m) of every cloud; returns the stage's cache in the
+        batch-1 view, {d: [1, b cap, C, 2d+1]}, and its node maxima [b cap]."""
+        b = self.b
+        if name not in self.stages:
+            self.stages[name] = ({d: t.new_empty((b, self.cap) + tuple(t.shape[2:])) for d, t in x.items()},
+                                 torch.empty((b, self.cap), dtype=torch.float32, device=self.coors.device))
+        feats, nodemax = self.stages[name]
+        for d, t in x.items():
+            feats[d][:, n0:n0 + m] = t.view((b, m) + tuple(t.shape[2:]))
+        nodemax[:, n0:n0 + m] = ops.node_absmax(x).view(b, m)
+        return {d: t.view((1, b * self.cap) + tuple(t.shape[2:])) for d, t in feats.items()}, nodemax.view(-1)
+
+    def _conv(self, conv, name, x, step):
+        """conv over the step's edges, its neighbours gathered from the cache of stage `name`, to which x is appended first."""
+        src, nodemax = self._append(name, x, step['n0'], step['m'])
+        edge_info, rel_dist, geom, rows = step['edge_info'], step['rel_dist'], step['geom'], step['rows']
+        d = conv_decide(conv, edge_info[0].numel(), rel_dist, geom)
+        sx = self._edge_scale([d], nodemax, edge_info[0])
+        self_out = conv.self_interact(x) if conv.self_interaction else None
+        return conv_forward([conv], rows.src(src), edge_info, rel_dist, (None, None, geom), decisions=[d], self_out=self_out, sx=sx)[0]
+
+    def _edge_scale(self, decisions, nodemax, idx):
+        """chunk_edge_scale from the cached node maxima."""
+        if not any(d.route == 'production' for d in decisions):
+            return None
+        return ops.edge_scale(None, idx, max(di for di, _ in decisions[0].conv.fiber_in), nodemax=nodemax).view(idx.shape)
+
+    def _attend(self, i, block, x, step, pos_emb):
+        attn = block.attn
+        features = block.prenorm(x)
+        src, nodemax = self._append(('attn', i), features, step['n0'], step['m'])
+        node_keys = None
+        if attn.linear_proj_keys:
+            node_keys = self._append(('keys', i), attn.to_k(features), step['n0'], step['m'])[0]
+        edge_info, rel_dist, geom, rows = step['edge_info'], step['rel_dist'], step['geom'], step['rows']
+        queries, kv, k_emb = attn.node_level(features, None, pos_emb, node_keys=node_keys)
+        decisions = [conv_decide(conv, edge_info[0].numel(), rel_dist, geom) for conv in attn.edge_convs()]
+        sx = self._edge_scale(decisions, nodemax, edge_info[0])
+        outputs = attn._attend(rows, src, queries, kv, k_emb, edge_info, rel_dist, (None, None, geom), decisions,
+                               attn.fuse_rotation(geom), sx)
+        return attn.project_out(outputs, x)
+
+    def _step(self, feats, coors, mask, edges, neighbor_mask, return_type, m):
+        """One extend (idempotent until self.n moves, so that a low-rank plan miss can run it again): (outputs, deferred checks)."""
+        model, b = self.model, self.b
+        n0, n1 = self.n, self.n + m
+        out_dtype = model._compute_dtype(coors)
+        if model.output_degrees == 1:
+            return_type = 0
+        dev = coors.device
+        positions = torch.arange(n0, n1, device=dev)
+        feats = model._embed_tokens(feats, positions)
+        if torch.is_tensor(feats):
+            feats = {'0': feats[..., None]}
+        if exists(edges) and edges.is_floating_point():
+            edges = edges.float()
+        feats = model._check_features(feats, coors)
+        self._grow(n1, dev)
+        self.coors[:, n0:n1] = coors.float()
+        self.mask[:, n0:n1] = True if mask is None else mask.to(dev, torch.bool)
+        k = model._num_neighbors(n1, 0)
+        idx, nmask, rel_pos, rel_dist = ops.knn_rows(self.coors, n1, n0, m, k, model._valid_radius(), node_mask=self.mask,
+                                                     neighbor_mask=None if neighbor_mask is None else neighbor_mask.to(dev),
+                                                     causal=True)
+        edge_values = None
+        if exists(edges):
+            edges = edges.to(dev)
+            edge_values = edges.gather(2, idx) if exists(model.edge_emb) else \
+                edges.gather(2, idx[..., None].expand(-1, -1, -1, edges.shape[-1]))
+        e = model._edge_features(edge_values, None)
+        pos_emb = None
+        if exists(model.rotary_pos_emb):
+            q_pos = positions.view(1, m).expand(b, m)
+            pos_emb = model._rotary(q_pos.reshape(1, b * m), torch.cat((q_pos[..., None], idx), dim=2).view(1, b * m, 1 + k), n1,
+                                    rel_dist.view(1, b * m, k))
+        # the batch-1 view: new row (c, i) is row c m + i, cached node (c, j) is node c cap + j
+        gidx = (idx + (torch.arange(b, device=dev) * self.cap).view(b, 1, 1)).view(1, b * m, k)
+        flat = lambda t: None if t is None else t.reshape((1, b * m) + tuple(t.shape[2:]))
+        geom = Geometry(flat(rel_pos), model.num_degrees - 1, deferred=[])
+        step = dict(n0=n0, m=m, rows=_StepRows(b * m), edge_info=(gidx, flat(nmask), flat(e)), rel_dist=flat(rel_dist), geom=geom)
+        x = self._conv(model.conv_in, 'in', {d: flat(t) for d, t in feats.items()}, step)
+        for i, (conv, nonlin) in enumerate(model.convs):
+            x = self._conv(conv, ('conv', i), nonlin(x), step)
+        for i, (attn_block, ff) in enumerate(model.net.blocks):
+            x = ff(self._attend(i, attn_block, x, step, pos_emb))
+        if exists(model.conv_out):
+            x = self._conv(model.conv_out, 'out', x, step)
+        out = model._output(x, lambda v: v.view((b, m) + tuple(v.shape[2:])), out_dtype, return_type)
+        return out, geom.deferred

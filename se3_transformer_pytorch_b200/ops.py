@@ -24,6 +24,7 @@ _SIGNATURES = {
     'se3_last_error': (ctypes.c_char_p, []),
     'se3_abi_version': (c_int, []),
     'se3_knn_fwd': (c_int, [c_void_p] * 7 + [c_int, c_int64, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
+    'se3_knn_rows_fwd': (c_int, [c_void_p] * 3 + [c_int, c_int64, c_int64, c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 5),
     'se3_pair_lookup_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
@@ -53,6 +54,10 @@ _SIGNATURES = {
     'se3_zgemm_image_bytes': (c_int64, [c_int, c_int, c_int]),
     'se3_zgemm_pack': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_zgemm_fwd': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_int64, c_int, c_int, c_int, c_void_p]),
+    'se3_zgemm_split_units': (c_int, [c_void_p, c_int, c_int, c_int, c_int]),
+    'se3_zgemm_workspace_bytes': (c_int64, [c_void_p, c_int, c_int64, c_int, c_int, c_int]),
+    'se3_zgemm_split_fwd': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_int64, c_int, c_int, c_int,
+                                    c_int, c_void_p, c_int64, c_void_p]),
     'se3_pool_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int64, c_void_p, c_void_p]),
     'se3_norm_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_float, c_int, c_void_p, c_void_p]),
     'se3_attn_aligned_fwd': (c_int, [c_void_p] * 4 + [c_int] + [c_void_p] * 7 + [c_int, c_void_p] + [c_int] * 7 + [c_float, c_void_p, c_void_p]),
@@ -271,6 +276,31 @@ def knn(coors, k, valid_radius, *, node_mask=None, neighbor_mask=None, sparse_ad
     with torch.cuda.device(dev), _timed('knn' if seqlens is None else 'knn_varlen', nbytes=nbytes):
         _check(lib().se3_knn_fwd(_p(coors), _p(cu), _p(kc), _p(off), _p(nm), *args, b, n, K, valid_radius, int(bool(causal)),
                                  _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
+    return idx, mask.view(torch.bool), rel_pos, rel_dist
+
+
+def knn_rows(coors, n, row0, m, k, valid_radius, *, node_mask=None, neighbor_mask=None, causal=False):
+    """The neighbour search of rows row0 .. row0 + m of clouds stored with room to grow: coors [b, ld, 3] and node_mask [b, ld]
+    (contiguous, ld >= n) hold b clouds of which the first n nodes are searched; neighbor_mask [b, m, n] holds the new rows'
+    masks.  Returns idx int64 [b, m, k] (local indices), mask bool [b, m, k], rel_pos [b, m, k, 3], rel_dist [b, m, k]: the rows
+    of knn() over the same b clouds of n nodes, bit for bit."""
+    _require_cuda(coors, node_mask, neighbor_mask)
+    if coors.dtype != torch.float32 or not coors.is_contiguous() or coors.dim() != 3:
+        raise ValueError('knn_rows: coors must be a contiguous float32 [b, ld, 3] tensor')
+    b, ld, _ = coors.shape
+    if node_mask is not None and (node_mask.shape != (b, ld) or not node_mask.is_contiguous()):
+        raise ValueError(f'knn_rows: node_mask must be a contiguous [b, ld] = {(b, ld)} tensor, got {tuple(node_mask.shape)}')
+    if neighbor_mask is not None and neighbor_mask.shape != (b, m, n):
+        raise ValueError(f'knn_rows: neighbor_mask must be [b, m, n] = {(b, m, n)}, got {tuple(neighbor_mask.shape)}')
+    dev = coors.device
+    idx = torch.empty((b, m, k), dtype=torch.int64, device=dev)
+    mask = torch.empty((b, m, k), dtype=torch.uint8, device=dev)
+    rel_pos = torch.empty((b, m, k, 3), dtype=torch.float32, device=dev)
+    rel_dist = torch.empty((b, m, k), dtype=torch.float32, device=dev)
+    nm, nbr = _u8(node_mask), _u8(neighbor_mask)
+    with torch.cuda.device(dev), _timed('knn_rows', nbytes=12 * b * n + 25 * b * m * k):
+        _check(lib().se3_knn_rows_fwd(_p(coors), _p(nm), _p(nbr), b, n, ld, row0, m, k, float(min(valid_radius, 3.0e38)),
+                                      int(bool(causal)), _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
     return idx, mask.view(torch.bool), rel_pos, rel_dist
 
 
@@ -648,16 +678,27 @@ def rotate_pool(Op, D, mask, self_add, nodes, K, Co, lo, out):
         _check(lib().se3_rotate_pool_fwd(_p(Op), _p(D), _p(_u8(mask)), _p(self_add), nodes, K, Co, lo, _p(out), _stream()))
 
 
-def edge_scale(feats, idx, max_degree):
-    """Power-of-two scale per edge from the largest |component| of the neighbour's features (all degrees): [E] fp32."""
-    b, n, k = idx.shape
+def node_absmax(feats):
+    """The largest |component| of every node's features over all degrees: feats {d: [b, n, C, 2d+1]} -> [b * n] fp32."""
     first = True
-    nodemax = torch.empty(b * n, dtype=torch.float32, device=idx.device)
+    for t in feats.values():
+        t = _f32(t)
+        if first:
+            rows = t.shape[0] * t.shape[1]
+            nodemax = torch.empty(rows, dtype=torch.float32, device=t.device)
+        with torch.cuda.device(t.device):
+            _check(lib().se3_rowabsmax_fwd(_p(t), rows, t.shape[2] * t.shape[3], int(not first), _p(nodemax), _stream()))
+        first = False
+    return nodemax
+
+
+def edge_scale(feats, idx, max_degree, nodemax=None):
+    """Power-of-two scale per edge from the largest |component| of the neighbour's features (all degrees): [E] fp32.  With
+    nodemax (node_absmax of every node idx addresses, [b * n]) feats is not read."""
+    b, n, k = idx.shape
+    if nodemax is None:
+        nodemax = node_absmax(feats)
     with torch.cuda.device(idx.device):
-        for t in feats.values():
-            t = _f32(t)
-            _check(lib().se3_rowabsmax_fwd(_p(t), b * n, t.shape[2] * t.shape[3], int(not first), _p(nodemax), _stream()))
-            first = False
         sx = torch.empty(b * n * k, dtype=torch.float32, device=idx.device)
         _check(lib().se3_edge_scale_fwd(_p(nodemax), _p(idx.contiguous()), b, n, k, max_degree, _p(sx), _stream()))
     return sx
@@ -733,8 +774,31 @@ def zgemm_image(parts, Co, mode):
     return img, S
 
 
-def zgemm(segs, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off, flush_stages=0, alg_flops=0, tag=''):
-    """segs: [(U [E,64] view (row stride 64; column offset folded into the pointer), X buffer, Ci, ncomp, cplus, cminus)]."""
+SPLIT_LAUNCHES = 0    # zgemm launches of this process that ran split-K (k_split > 1)
+_SMS = {}
+
+
+def sm_count(device):
+    """Streaming multiprocessors of `device`."""
+    key = torch.device(device).index if torch.device(device).index is not None else torch.cuda.current_device()
+    if key not in _SMS:
+        _SMS[key] = torch.cuda.get_device_properties(key).multi_processor_count
+    return _SMS[key]
+
+
+def zgemm_k_split(tiles, units, sms):
+    """CTAs per output tile of a zgemm launch with `tiles` output tiles and `units` split units on a card of `sms` SMs: 1 when the
+    unsplit grid already has a CTA per SM, else as many as fit one wave, at most one unit each."""
+    if tiles >= sms:
+        return 1
+    return max(1, min(units, sms // tiles))
+
+
+def zgemm(segs, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off, flush_stages=0, alg_flops=0, tag='', k_split=None):
+    """segs: [(U [E,64] view (row stride 64; column offset folded into the pointer), X buffer, Ci, ncomp, cplus, cminus)].
+    k_split: CTAs per output tile (split-K over whole drain / Gauss blocks, bit-identical to 1); None chooses it from the grid,
+    the launch's split units and the SM count (zgemm_k_split).  A forced value above the launch's units is refused."""
+    global SPLIT_LAUNCHES
     _require_cuda(w_img, sx, out)
     arr = (ZSeg * len(segs))()
     Ktot = 0
@@ -749,9 +813,22 @@ def zgemm(segs, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off, flush_st
     mma = 2 * E * Co * Ktot * 3 * (2 if mode == 2 else 1)
     planes = 1 if mode == 1 else 2
     nbytes = w_img.numel() + 4 * E * Co * planes + sum(4 * E * s[2] * (planes + 16) for s in segs)
-    with torch.cuda.device(out.device), _timed('zgemm', flops=alg_flops, nbytes=nbytes, tag=tag or f'mode{mode}N{N}K{Ktot}', mma=mma):
-        _check(lib().se3_zgemm_fwd(arr, len(segs), _p(w_img), _p(sx), E, Co, mode, _p(out), out_edge_stride, comp_off[0],
-                                   comp_off[1] if len(comp_off) > 1 else 0, flush_stages, _stream()))
+    units = lib().se3_zgemm_split_units(arr, len(segs), Co, mode, flush_stages)
+    if units < 1:
+        raise ValueError(f'zgemm: unsupported launch (Co={Co}, mode={mode}, {len(segs)} segments)')
+    if k_split is None:
+        k_split = zgemm_k_split(((E + TILE_E - 1) // TILE_E) * (Co // (64 if mode == 2 else 128)), units, sm_count(out.device))
+    elif not 1 <= k_split <= units:
+        raise ValueError(f'zgemm: k_split = {k_split} outside [1, {units}], the split units (drain / Gauss blocks) of this launch')
+    ws, ws_bytes = None, 0
+    if k_split > 1:
+        ws_bytes = lib().se3_zgemm_workspace_bytes(arr, len(segs), E, Co, mode, flush_stages)
+        ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=out.device)
+        SPLIT_LAUNCHES += 1
+    tag = (tag or f'mode{mode}N{N}K{Ktot}') + (f'split{k_split}' if k_split > 1 else '')
+    with torch.cuda.device(out.device), _timed('zgemm', flops=alg_flops, nbytes=nbytes, tag=tag, mma=mma):
+        _check(lib().se3_zgemm_split_fwd(arr, len(segs), _p(w_img), _p(sx), E, Co, mode, _p(out), out_edge_stride, comp_off[0],
+                                         comp_off[1] if len(comp_off) > 1 else 0, flush_stages, k_split, _p(ws), ws_bytes, _stream()))
 
 
 # max-abs residual of the radial basis relative to max|G|.  The fp32 trunk itself carries ~6e-7..1e-6 of rounding noise
