@@ -90,6 +90,20 @@ int se3_knn_rows_fwd(const float* coors, const uint8_t* node_mask, const uint8_t
                      int row0, int nrows, int k, float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask,
                      float* out_rel_pos, float* out_rel_dist, void* stream);
 
+/* The same search for the new rows of num_clouds clouds of different lengths, each growing on its own (packed causal decoding).
+ * coors [S, ld, 3] holds cloud c in row slot[c]; its m_c = cu_rows[c + 1] - cu_rows[c] new rows are nodes n_prev[c] + r,
+ * searched over its first n_cur_c = n_prev[c] + m_c nodes for k_per_cloud[c] neighbours.  neighbor_mask (may be NULL) holds
+ * the new rows' [m_c, n_cur_c] uint8 masks end to end, cloud c's from pair_off[c] (pair_off[c] < 0: that cloud has none).
+ * Outputs [rows, K] (rel_pos [rows, K, 3]) with rows = cu_rows[num_clouds]; indices are slot[c] * ld + j, and slots r >= k_c
+ * repeat slot k_c - 1 with mask 0.  n_max = max n_cur_c sizes shared memory.  Every descriptor is int64 on the device and is
+ * read by the kernel only, so the call does not synchronise: the caller guarantees cu_rows[0] = 0, m_c >= 1, n_cur_c in
+ * [2, n_max], 1 <= k_c <= min(n_cur_c - 1, K), slot[c] in [0, S) and masks inside the buffer.  Row r of cloud c is bit for
+ * bit row n_prev[c] + r that se3_knn_rows_fwd writes for that cloud alone with n = n_cur_c and k = k_c (slots < k_c). */
+int se3_knn_rows_packed_fwd(const float* coors, const uint8_t* neighbor_mask, const int64_t* cu_rows, const int64_t* slot,
+                            const int64_t* n_prev, const int64_t* k_per_cloud, const int64_t* pair_off, int num_clouds, int64_t rows,
+                            int64_t ld, int n_max, int K, float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask,
+                            float* out_rel_pos, float* out_rel_dist, void* stream);
+
 /* Position of every neighbour in a sparse pair list (as in se3_pairs; batch_stride 0 when shared, else n): out[b,i,kk] = p with
  * cols[p] == idx[b,i,kk] inside row (b, i), or -1 if the row lacks that column.  idx, out: [b, n, k] int64.  The caller indexes
  * the list's values (edge tokens, edge features, hop counts) with a zero row appended for -1. */

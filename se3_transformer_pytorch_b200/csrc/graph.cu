@@ -246,22 +246,49 @@ knn_kernel(const float* __restrict__ coors, const int64_t* __restrict__ cu_seqle
                    out_rel_dist + o);
 }
 
-// One CTA per new row (cloud c, node i = row0 + r) of clouds that grow one step at a time: rows [row0, row0 + nrows) of b clouds
-// whose first n nodes are searched, stored with a leading dimension of ld >= n nodes (coors [b, ld, 3], node_mask [b, ld]);
-// nbr [b, nrows, n] holds the new rows' byte masks.  The row body is knn_row, so the results are those of knn_kernel's rows.
+// One CTA per new row of clouds that grow one step at a time, stored with a leading dimension of ld nodes (coors [rows, ld, 3],
+// node_mask [rows, ld]).  Uniform clouds (cu_rows NULL): rows [row0, row0 + nrows) of b clouds whose first n nodes are searched
+// for k neighbours, nbr [b, nrows, n] the new rows' byte masks, indices local to the cloud.  Ragged clouds: the CTA finds its
+// cloud c by binary search in cu_rows, as knn_kernel does in cu_seqlens; its row r is node n_prev[c] + r of the cloud in store
+// row slot[c], searched over its first n_prev[c] + m_c nodes for k_per_cloud[c] neighbours into k >= k_c slots; its byte mask
+// row starts at nbr + pair_off[c] + r (n_prev[c] + m_c) (pair_off[c] < 0: no mask); indices are slot[c] ld + j.  The row body
+// is knn_row, so the results are those of knn_kernel's rows.
 template <int THREADS>
 __global__ void __launch_bounds__(THREADS, 6)
-knn_rows_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mask, const uint8_t* __restrict__ nbr, int n,
-                int64_t ld, int row0, int nrows, int k, float valid_radius, int causal, int64_t* __restrict__ out_idx,
+knn_rows_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ node_mask, const uint8_t* __restrict__ nbr,
+                const int64_t* __restrict__ cu_rows, const int64_t* __restrict__ slot, const int64_t* __restrict__ n_prev,
+                const int64_t* __restrict__ k_per_cloud, const int64_t* __restrict__ pair_off, int num_clouds, int n, int64_t ld,
+                int row0, int nrows, int k, float valid_radius, int causal, int64_t* __restrict__ out_idx,
                 uint8_t* __restrict__ out_mask, float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
   extern __shared__ unsigned long long keys[];
   const int64_t t = blockIdx.x;
-  const int64_t c = t / nrows;
-  const int i = row0 + (int)(t % nrows);
-  const DensePairs pairs{nbr ? nbr + t * n : nullptr, nullptr};
+  int64_t c, j_base = 0;
+  int i, n_c, k_c;
+  const uint8_t* row_mask;
+  if (cu_rows) {
+    int lo = 0, hi = num_clouds - 1;                // the last cloud with cu_rows[lo] <= t
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (cu_rows[mid] <= t) lo = mid; else hi = mid - 1;
+    }
+    const int64_t r = t - cu_rows[lo];
+    c = slot[lo];
+    i = (int)(n_prev[lo] + r);
+    n_c = (int)(n_prev[lo] + cu_rows[lo + 1] - cu_rows[lo]);
+    k_c = (int)k_per_cloud[lo];
+    row_mask = nbr && pair_off[lo] >= 0 ? nbr + pair_off[lo] + r * n_c : nullptr;
+    j_base = c * ld;
+  } else {
+    c = t / nrows;
+    i = row0 + (int)(t % nrows);
+    n_c = n;
+    k_c = k;
+    row_mask = nbr ? nbr + t * n : nullptr;
+  }
   const int64_t o = t * k;
-  knn_row<THREADS>(keys, coors + c * ld * 3, n, i, k, knn_npad(n), pairs, node_mask ? node_mask + c * ld : nullptr, valid_radius,
-                   causal, k, 0, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
+  knn_row<THREADS>(keys, coors + c * ld * 3, n_c, i, k_c, knn_npad(n_c), DensePairs{row_mask, nullptr},
+                   node_mask ? node_mask + c * ld : nullptr, valid_radius, causal, k, j_base, out_idx + o, out_mask + o,
+                   out_rel_pos + o * 3, out_rel_dist + o);
 }
 
 __global__ void gather_pairs_kernel(const float* __restrict__ pf, const int64_t* __restrict__ idx, int n, int k, int e,
@@ -375,6 +402,25 @@ extern "C" int se3_knn_fwd(const float* coors, const int64_t* cu_seqlens, const 
   return csr ? launch(knn_kernel<THREADS, CsrPairs>) : launch(knn_kernel<THREADS, DensePairs>);
 }
 
+namespace se3 {
+// knn_rows_kernel over `rows` CTAs; n: the longest searched cloud, which sizes shared memory (K slots per row)
+static int launch_knn_rows(const float* coors, const uint8_t* node_mask, const uint8_t* nbr, const int64_t* cu_rows,
+                           const int64_t* slot, const int64_t* n_prev, const int64_t* k_per_cloud, const int64_t* pair_off,
+                           int num_clouds, int n, int64_t ld, int row0, int nrows, int64_t rows, int K, float valid_radius, int causal,
+                           int64_t* out_idx, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream) {
+  constexpr int THREADS = 256;
+  const int key_words = n - 1 > KNN_TILE ? KNN_TILE + next_pow2(K) : knn_npad(n);
+  const size_t smem = (size_t)key_words * sizeof(unsigned long long);
+  auto kernel = knn_rows_kernel<THREADS>;
+  if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)rows, THREADS, smem, as_stream(stream)>>>(coors, node_mask, nbr, cu_rows, slot, n_prev, k_per_cloud, pair_off,
+                                                               num_clouds, n, ld, row0, nrows, K, valid_radius, causal, out_idx,
+                                                               out_mask, out_rel_pos, out_rel_dist);
+  SE3_LAUNCH_OK();
+  return SE3_OK;
+}
+}  // namespace se3
+
 extern "C" int se3_knn_rows_fwd(const float* coors, const uint8_t* node_mask, const uint8_t* neighbor_mask, int b, int64_t n, int64_t ld,
                                 int row0, int nrows, int k, float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask,
                                 float* out_rel_pos, float* out_rel_dist, void* stream) {
@@ -387,16 +433,24 @@ extern "C" int se3_knn_rows_fwd(const float* coors, const uint8_t* node_mask, co
   SE3_REQUIRE(k >= 1 && k <= n - 1 && k <= KNN_TILE, "se3_knn_rows_fwd: k must be in [1, min(n-1, %d)] (got k=%d n=%lld)", KNN_TILE, k,
               (long long)n);
   SE3_REQUIRE((int64_t)b * nrows < (1ll << 31), "se3_knn_rows_fwd: %lld rows exceed the 1-D grid", (long long)b * nrows);
-  constexpr int THREADS = 256;
-  const int key_words = n - 1 > KNN_TILE ? KNN_TILE + next_pow2(k) : knn_npad((int)n);
-  const size_t smem = (size_t)key_words * sizeof(unsigned long long);
-  auto kernel = knn_rows_kernel<THREADS>;
-  if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kernel<<<(unsigned)((int64_t)b * nrows), THREADS, smem, as_stream(stream)>>>(coors, node_mask, neighbor_mask, (int)n, ld, row0, nrows,
-                                                                              k, valid_radius, causal, out_idx, out_mask, out_rel_pos,
-                                                                              out_rel_dist);
-  SE3_LAUNCH_OK();
-  return SE3_OK;
+  return launch_knn_rows(coors, node_mask, neighbor_mask, nullptr, nullptr, nullptr, nullptr, nullptr, 0, (int)n, ld, row0, nrows,
+                         (int64_t)b * nrows, k, valid_radius, causal, out_idx, out_mask, out_rel_pos, out_rel_dist, stream);
+}
+
+extern "C" int se3_knn_rows_packed_fwd(const float* coors, const uint8_t* neighbor_mask, const int64_t* cu_rows, const int64_t* slot,
+                                       const int64_t* n_prev, const int64_t* k_per_cloud, const int64_t* pair_off, int num_clouds,
+                                       int64_t rows, int64_t ld, int n_max, int K, float valid_radius, int causal, int64_t* out_idx,
+                                       uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream) {
+  using namespace se3;
+  SE3_REQUIRE(coors && cu_rows && slot && n_prev && k_per_cloud && out_idx && out_mask && out_rel_pos && out_rel_dist,
+              "se3_knn_rows_packed_fwd: null pointer");
+  SE3_REQUIRE(!neighbor_mask || pair_off, "se3_knn_rows_packed_fwd: a neighbour mask needs pair_off");
+  SE3_REQUIRE(num_clouds > 0 && rows >= num_clouds && rows < (1ll << 31),
+              "se3_knn_rows_packed_fwd: need 0 < num_clouds <= rows < 2^31 (got %d clouds, %lld rows)", num_clouds, (long long)rows);
+  SE3_REQUIRE(n_max > 1 && n_max <= ld, "se3_knn_rows_packed_fwd: need 1 < n_max <= ld (got n_max=%d ld=%lld)", n_max, (long long)ld);
+  SE3_REQUIRE(K >= 1 && K <= KNN_TILE, "se3_knn_rows_packed_fwd: K must be in [1, %d] (got %d)", KNN_TILE, K);
+  return launch_knn_rows(coors, nullptr, neighbor_mask, cu_rows, slot, n_prev, k_per_cloud, pair_off, num_clouds, n_max, ld, 0, 1,
+                         rows, K, valid_radius, causal, out_idx, out_mask, out_rel_pos, out_rel_dist, stream);
 }
 
 extern "C" int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx,

@@ -1393,6 +1393,11 @@ class SE3Transformer(nn.Module):
         doing the edge work of its new nodes only."""
         return CausalDecoder(self, batch_size)
 
+    def packed_decoder(self):
+        """An empty PackedCausalDecoder of this causal model: clouds of different lengths decoded together, each opened, extended,
+        truncated, forked and closed on its own, every step carrying the new nodes of any subset of them."""
+        return PackedCausalDecoder(self)
+
     # ---- forward ----------------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, feats, coors, mask=None, adj_mat=None, edges=None, return_type=None, return_pooled=False,
@@ -1927,9 +1932,9 @@ FLT_MAX = 3.4028234663852886e38
 
 
 class _StepRows:
-    """The node chunk of a CausalDecoder step, in the batch-1 view with global indices that forward_packed uses: its rows are
+    """The node chunk of a decoding step, in the batch-1 view with global indices that forward_packed uses: its rows are
     the step's new nodes (row-level tensors are passed as they are) and its neighbours are gathered from the decoder's cache,
-    a [1, b * capacity, ...] tensor of which src() gives the view the kernels expect (NodeChunk.src)."""
+    a [1, rows * capacity, ...] tensor of which src() gives the view the kernels expect (NodeChunk.src)."""
     b0, b1, whole = 0, 1, False
 
     def __init__(self, rows):
@@ -1947,50 +1952,133 @@ class _StepRows:
         return t[:, :self.n_rows]
 
 
-class CausalDecoder:
-    """Generation with a causal SE3Transformer, node by node (SE3Transformer.causal_decoder).
+def _refuse_undecodable(model, api):
+    """The models whose outputs cannot be decoded from a cache of earlier rows, refused with the reason (both decoders)."""
+    if not model.causal:
+        raise ValueError(f'{api}: the model is not causal (causal=False): the outputs of earlier nodes would change as '
+                         'nodes arrive, so they cannot be cached')
+    if model.attend_sparse_neighbors or exists(model.num_adj_degrees):
+        raise NotImplementedError(f'{api}: attend_sparse_neighbors and num_adj_degrees are not supported: the number of '
+                                  'bonded neighbours and the hop counts depend on the whole adjacency, including future rows')
+    if model.accept_global_feats:
+        raise NotImplementedError(f'{api}: models built with global_feats_dim are not supported (the attention kernel '
+                                  'indexes the global keys by batch row, and a decoding step is one row)')
+    if not model.valid_radius < FLT_MAX:
+        raise ValueError(f'{api}: valid_radius = {model.valid_radius} >= FLT_MAX: the FLT_MAX keys of later nodes would '
+                         'count as valid neighbours, so even forward() is not causal; give a finite radius below FLT_MAX')
+
+
+class _DecoderStages:
+    """What CausalDecoder and PackedCausalDecoder share: the per-stage cache and the walk of a step through the stages once its
+    graph is built.
 
     Node i of a causal model depends only on nodes j <= i: the neighbour search gives every later column the key FLT_MAX, so
     later nodes only fill masked slots, which get zero weight in the attention softmax and in the pooled means; everything else
-    is per node.  The decoder therefore keeps, per cloud and per stage, the node features that later nodes gather as neighbours
+    is per node.  A decoder therefore keeps, per cloud and per stage, the node features that later nodes gather as neighbours
     (the embedded input of conv_in, the input of each pre-convolution, prenorm(x) of every attention block and its node keys
-    with linear_proj_keys, the input of conv_out), with their node maxima (the production route's edge scales), in storage that
-    grows geometrically.  extend() searches the neighbours of the new rows only, runs every convolution and attention block over
-    the new nodes' edges and the node-level work over the new rows, and appends the new rows to the cache.
+    with linear_proj_keys, the input of conv_out), with their node maxima (the production route's edge scales), in tensors
+    [rows, cap, ...] whose row r holds one cloud.  A step searches the neighbours of the new rows only, runs every convolution
+    and attention block over the new nodes' edges and the node-level work over the new rows, and stores the new rows in the
+    cache.  A subclass builds the step's graph and says where its new rows go (_store)."""
 
-    extend(feats, coors, ...) returns rows [n_prev, n_cur) of what forward returns for all nodes so far, with the [b, n, n] pair
-    inputs stacked from the rows given (anything above the diagonal).  The first call (the prefill) needs at least 2 nodes, as a
-    forward does.  Lockstep batches: every call adds the same number of nodes to each of the batch_size clouds."""
+    row_bytes = 12                                # cache bytes per node besides the stages: the coordinates
 
-    def __init__(self, model, batch_size=1):
-        if not model.causal:
-            raise ValueError('causal_decoder: the model is not causal (causal=False): the outputs of earlier nodes would change as '
-                             'nodes arrive, so they cannot be cached')
-        if model.attend_sparse_neighbors or exists(model.num_adj_degrees):
-            raise NotImplementedError('causal_decoder: attend_sparse_neighbors and num_adj_degrees are not supported: the number of '
-                                      'bonded neighbours and the hop counts depend on the whole adjacency, including future rows')
-        if model.accept_global_feats:
-            raise NotImplementedError('causal_decoder: models built with global_feats_dim are not supported (the attention kernel '
-                                      'indexes the global keys by batch row, and a decoding step is one row)')
-        if not model.valid_radius < FLT_MAX:
-            raise ValueError(f'causal_decoder: valid_radius = {model.valid_radius} >= FLT_MAX: the FLT_MAX keys of later nodes would '
-                             'count as valid neighbours, so even forward() is not causal; give a finite radius below FLT_MAX')
-        if operator.index(batch_size) < 1:
-            raise ValueError(f'causal_decoder: batch_size must be >= 1, got {batch_size}')
-        self.model, self.b = model, int(batch_size)
-        self.n = self.cap = 0
-        self.coors = self.mask = None             # [b, cap, 3] fp32, [b, cap] bool
-        self.stages = {}                          # name -> (feats {d: [b, cap, C, 2d+1]}, nodemax [b, cap])
-
-    def __len__(self):
-        return self.n
+    def __init__(self, model, api):
+        _refuse_undecodable(model, api)
+        self.model = model
+        self.cap = 0
+        self.coors = None                         # [rows, cap, 3] fp32
+        self.stages = {}                          # name -> (feats {d: [rows, cap, C, 2d+1]}, nodemax [rows, cap])
 
     def cache_bytes_per_node(self):
-        """Bytes the cache holds per node of a cloud (features, node maxima, coordinates and mask)."""
-        per = 13
+        """Bytes the cache holds per node of a cloud (features, node maxima, coordinates and, with a node mask, the mask)."""
+        per = self.row_bytes
         for feats, nodemax in self.stages.values():
             per += sum(t[0, 0].numel() * 4 for t in feats.values()) + 4
         return per
+
+    def _store(self, cache, rows, step):
+        """Write the step's new rows [R, ...] into their places in cache [rows, cap, ...]."""
+        raise NotImplementedError
+
+    def _append(self, name, x, step):
+        """Store the new rows x {d: [1, R, C, 2d+1]} of stage `name`; returns the stage's cache in the batch-1 view,
+        {d: [1, rows cap, C, 2d+1]}, and its node maxima [rows cap]."""
+        if name not in self.stages:
+            shape = tuple(self.coors.shape[:2])
+            self.stages[name] = ({d: t.new_empty(shape + tuple(t.shape[2:])) for d, t in x.items()},
+                                 torch.empty(shape, dtype=torch.float32, device=self.coors.device))
+        feats, nodemax = self.stages[name]
+        for d, t in x.items():
+            self._store(feats[d], t[0], step)
+        self._store(nodemax, ops.node_absmax(x).view(-1), step)
+        return {d: t.view((1, -1) + tuple(t.shape[2:])) for d, t in feats.items()}, nodemax.view(-1)
+
+    def _conv(self, conv, name, x, step):
+        """conv over the step's edges, its neighbours gathered from the cache of stage `name`, to which x is appended first."""
+        src, nodemax = self._append(name, x, step)
+        edge_info, rel_dist, geom, rows = step['edge_info'], step['rel_dist'], step['geom'], step['rows']
+        d = conv_decide(conv, edge_info[0].numel(), rel_dist, geom)
+        sx = self._edge_scale([d], nodemax, edge_info[0])
+        self_out = conv.self_interact(x) if conv.self_interaction else None
+        return conv_forward([conv], rows.src(src), edge_info, rel_dist, (None, None, geom), decisions=[d], self_out=self_out, sx=sx)[0]
+
+    def _edge_scale(self, decisions, nodemax, idx):
+        """chunk_edge_scale from the cached node maxima."""
+        if not any(d.route == 'production' for d in decisions):
+            return None
+        return ops.edge_scale(None, idx, max(di for di, _ in decisions[0].conv.fiber_in), nodemax=nodemax).view(idx.shape)
+
+    def _attend(self, i, block, x, step, pos_emb):
+        attn = block.attn
+        features = block.prenorm(x)
+        src, nodemax = self._append(('attn', i), features, step)
+        node_keys = None
+        if attn.linear_proj_keys:
+            node_keys = self._append(('keys', i), attn.to_k(features), step)[0]
+        edge_info, rel_dist, geom, rows = step['edge_info'], step['rel_dist'], step['geom'], step['rows']
+        queries, kv, k_emb = attn.node_level(features, None, pos_emb, node_keys=node_keys)
+        decisions = [conv_decide(conv, edge_info[0].numel(), rel_dist, geom) for conv in attn.edge_convs()]
+        sx = self._edge_scale(decisions, nodemax, edge_info[0])
+        outputs = attn._attend(rows, src, queries, kv, k_emb, edge_info, rel_dist, (None, None, geom), decisions,
+                               attn.fuse_rotation(geom), sx)
+        return attn.project_out(outputs, x)
+
+    def _walk(self, feats, step, pos_emb, reduce, out_dtype, return_type):
+        """Every stage of the trunk over the step's R new rows (feats {d: [1, R, C, 2d+1]}; step: the graph in the batch-1 view,
+        rows, edge_info, rel_dist and geom, and what _store needs): (outputs, deferred checks of the low-rank plans)."""
+        model = self.model
+        x = self._conv(model.conv_in, 'in', feats, step)
+        for i, (conv, nonlin) in enumerate(model.convs):
+            x = self._conv(conv, ('conv', i), nonlin(x), step)
+        for i, (attn_block, ff) in enumerate(model.net.blocks):
+            x = ff(self._attend(i, attn_block, x, step, pos_emb))
+        if exists(model.conv_out):
+            x = self._conv(model.conv_out, 'out', x, step)
+        return model._output(x, reduce, out_dtype, return_type), step['geom'].deferred
+
+
+class CausalDecoder(_DecoderStages):
+    """Generation with a causal SE3Transformer, node by node (SE3Transformer.causal_decoder); see _DecoderStages for what is
+    cached and why it is exact.  Lockstep batches: the cache row of cloud c is c, and every call adds the same number of nodes
+    to each of the batch_size clouds.
+
+    extend(feats, coors, ...) returns rows [n_prev, n_cur) of what forward returns for all nodes so far, with the [b, n, n] pair
+    inputs stacked from the rows given (anything above the diagonal).  The first call (the prefill) needs at least 2 nodes, as a
+    forward does."""
+
+    row_bytes = 13                                # coordinates and node mask
+
+    def __init__(self, model, batch_size=1):
+        super().__init__(model, 'causal_decoder')
+        if operator.index(batch_size) < 1:
+            raise ValueError(f'causal_decoder: batch_size must be >= 1, got {batch_size}')
+        self.b = int(batch_size)
+        self.n = 0
+        self.mask = None                          # [b, cap] bool
+
+    def __len__(self):
+        return self.n
 
     # ---- checks --------------------------------------------------------------------------------------------
     def _check(self, feats, coors, mask, edges, neighbor_mask, return_pooled):
@@ -2061,49 +2149,6 @@ class CausalDecoder:
         self.stages = {name: ({d: grown(t) for d, t in feats.items()}, grown(nodemax)) for name, (feats, nodemax) in self.stages.items()}
         self.cap = cap
 
-    def _append(self, name, x, n0, m):
-        """Store the new rows x {d: [1, b m, C, 2d+1]} of stage `name` at [n0, n0 + m) of every cloud; returns the stage's cache in the
-        batch-1 view, {d: [1, b cap, C, 2d+1]}, and its node maxima [b cap]."""
-        b = self.b
-        if name not in self.stages:
-            self.stages[name] = ({d: t.new_empty((b, self.cap) + tuple(t.shape[2:])) for d, t in x.items()},
-                                 torch.empty((b, self.cap), dtype=torch.float32, device=self.coors.device))
-        feats, nodemax = self.stages[name]
-        for d, t in x.items():
-            feats[d][:, n0:n0 + m] = t.view((b, m) + tuple(t.shape[2:]))
-        nodemax[:, n0:n0 + m] = ops.node_absmax(x).view(b, m)
-        return {d: t.view((1, b * self.cap) + tuple(t.shape[2:])) for d, t in feats.items()}, nodemax.view(-1)
-
-    def _conv(self, conv, name, x, step):
-        """conv over the step's edges, its neighbours gathered from the cache of stage `name`, to which x is appended first."""
-        src, nodemax = self._append(name, x, step['n0'], step['m'])
-        edge_info, rel_dist, geom, rows = step['edge_info'], step['rel_dist'], step['geom'], step['rows']
-        d = conv_decide(conv, edge_info[0].numel(), rel_dist, geom)
-        sx = self._edge_scale([d], nodemax, edge_info[0])
-        self_out = conv.self_interact(x) if conv.self_interaction else None
-        return conv_forward([conv], rows.src(src), edge_info, rel_dist, (None, None, geom), decisions=[d], self_out=self_out, sx=sx)[0]
-
-    def _edge_scale(self, decisions, nodemax, idx):
-        """chunk_edge_scale from the cached node maxima."""
-        if not any(d.route == 'production' for d in decisions):
-            return None
-        return ops.edge_scale(None, idx, max(di for di, _ in decisions[0].conv.fiber_in), nodemax=nodemax).view(idx.shape)
-
-    def _attend(self, i, block, x, step, pos_emb):
-        attn = block.attn
-        features = block.prenorm(x)
-        src, nodemax = self._append(('attn', i), features, step['n0'], step['m'])
-        node_keys = None
-        if attn.linear_proj_keys:
-            node_keys = self._append(('keys', i), attn.to_k(features), step['n0'], step['m'])[0]
-        edge_info, rel_dist, geom, rows = step['edge_info'], step['rel_dist'], step['geom'], step['rows']
-        queries, kv, k_emb = attn.node_level(features, None, pos_emb, node_keys=node_keys)
-        decisions = [conv_decide(conv, edge_info[0].numel(), rel_dist, geom) for conv in attn.edge_convs()]
-        sx = self._edge_scale(decisions, nodemax, edge_info[0])
-        outputs = attn._attend(rows, src, queries, kv, k_emb, edge_info, rel_dist, (None, None, geom), decisions,
-                               attn.fuse_rotation(geom), sx)
-        return attn.project_out(outputs, x)
-
     def _step(self, feats, coors, mask, edges, neighbor_mask, return_type, m):
         """One extend (idempotent until self.n moves, so that a low-rank plan miss can run it again): (outputs, deferred checks)."""
         model, b = self.model, self.b
@@ -2142,12 +2187,227 @@ class CausalDecoder:
         flat = lambda t: None if t is None else t.reshape((1, b * m) + tuple(t.shape[2:]))
         geom = Geometry(flat(rel_pos), model.num_degrees - 1, deferred=[])
         step = dict(n0=n0, m=m, rows=_StepRows(b * m), edge_info=(gidx, flat(nmask), flat(e)), rel_dist=flat(rel_dist), geom=geom)
-        x = self._conv(model.conv_in, 'in', {d: flat(t) for d, t in feats.items()}, step)
-        for i, (conv, nonlin) in enumerate(model.convs):
-            x = self._conv(conv, ('conv', i), nonlin(x), step)
-        for i, (attn_block, ff) in enumerate(model.net.blocks):
-            x = ff(self._attend(i, attn_block, x, step, pos_emb))
-        if exists(model.conv_out):
-            x = self._conv(model.conv_out, 'out', x, step)
-        out = model._output(x, lambda v: v.view((b, m) + tuple(v.shape[2:])), out_dtype, return_type)
-        return out, geom.deferred
+        return self._walk({d: flat(t) for d, t in feats.items()}, step, pos_emb, lambda v: v.view((b, m) + tuple(v.shape[2:])),
+                          out_dtype, return_type)
+
+    def _store(self, cache, rows, step):
+        """New row (c, i) goes to node n0 + i of cache row c."""
+        n0, m = step['n0'], step['m']
+        cache[:, n0:n0 + m] = rows.view((self.b, m) + tuple(rows.shape[1:]))
+
+
+class PackedCausalDecoder(_DecoderStages):
+    """Generation with a causal SE3Transformer for clouds of different lengths that join, leave, rewind and fork on their own
+    (SE3Transformer.packed_decoder); see _DecoderStages for what is cached and why it is exact.  Inputs and outputs follow
+    forward_packed: the nodes of a step are concatenated along one axis, with no batch padding and no node mask.
+
+    For every cloud, the rows returned across its extend calls are the rows of model(feats_c[None], coors_c[None], ...) over that
+    cloud's nodes so far (batch 1, no mask), whatever the other clouds of the same steps do, however its nodes were split into
+    calls, and across truncate, fork and the reuse of a closed cloud's cache row.  Each cloud has its own neighbour count
+    k_c = min(num_neighbors, n_cur_c - 1) in a step of K = max k_c slots (slots r >= k_c are masked), and positions and rotary
+    positions count from the cloud's first node.
+
+    The cache is [S, cap, ...] per stage: cloud c lives in row slot_c, and its node j at column j.  S doubles when more clouds
+    are open than there are rows and cap doubles when a cloud outgrows it; a row costs cap nodes whatever its cloud's length (no
+    paged cache).  Columns at or past a cloud's length are never read, so truncate only moves the length and close only frees
+    the row.  A step without pair inputs launches no device work per cloud; edges and neighbor_mask are concatenated from one
+    tensor per listed cloud."""
+
+    def __init__(self, model):
+        super().__init__(model, 'packed_decoder')
+        self.S = 0                                # cache rows allocated on the device
+        self._next_id = 0
+        self._slot, self._len = {}, {}            # open cloud id -> cache row, number of nodes
+
+    # ---- lifecycle -----------------------------------------------------------------------------------------
+    def open(self, count=1):
+        """count new empty clouds; returns their ids, increasing integers that are never reused."""
+        if operator.index(count) < 1:
+            raise ValueError(f'open: count must be >= 1, got {count}')
+        ids = []
+        for _ in range(int(count)):
+            used = set(self._slot.values())
+            slot = next(s for s in range(len(used) + 1) if s not in used)
+            ids.append(self._next_id)
+            self._slot[self._next_id], self._len[self._next_id] = slot, 0
+            self._next_id += 1
+        return ids
+
+    def close(self, cloud):
+        """Forget a cloud; its cache row is free for the next cloud that opens."""
+        self._known(cloud, 'close')
+        del self._slot[cloud], self._len[cloud]
+
+    def truncate(self, cloud, n):
+        """Rewind a cloud to its first n nodes (0 <= n <= length).  Exact: cached rows of nodes < n do not depend on later nodes."""
+        self._known(cloud, 'truncate')
+        n = operator.index(n)
+        if not 0 <= n <= self._len[cloud]:
+            raise ValueError(f'truncate: n must be in [0, {self._len[cloud]}] for cloud {cloud}, got {n}')
+        self._len[cloud] = n
+
+    @torch.no_grad()
+    def fork(self, cloud):
+        """A new cloud whose nodes so far are a copy of `cloud`'s (beam search, parallel sampling); returns its id."""
+        self._known(cloud, 'fork')
+        n, src = self._len[cloud], self._slot[cloud]
+        new = self.open()[0]
+        if n:
+            dst = self._slot[new]
+            self._grow(dst + 1, n, self.coors.device)
+            for t in [self.coors] + [t for feats, nodemax in self.stages.values() for t in (*feats.values(), nodemax)]:
+                t[dst, :n] = t[src, :n]
+            self._len[new] = n
+        return new
+
+    def length(self, cloud):
+        self._known(cloud, 'length')
+        return self._len[cloud]
+
+    def open_ids(self):
+        return sorted(self._slot)
+
+    def _known(self, cloud, api):
+        try:
+            if operator.index(cloud) in self._slot:
+                return
+        except TypeError:
+            pass
+        raise ValueError(f'{api}: {cloud!r} is not an open cloud of this decoder (open: {self.open_ids()[:16]})')
+
+    # ---- checks --------------------------------------------------------------------------------------------
+    def _check(self, ids, seqlens, feats, coors, edges, neighbor_mask, return_pooled):
+        """Everything extend takes from the caller, checked before any device work; returns (ids, seqlens) as lists of ints."""
+        model = self.model
+        if return_pooled:
+            raise ValueError('extend: return_pooled is not supported: the mean over nodes changes with every node that arrives')
+        try:
+            ids, seqlens = [operator.index(c) for c in ids], [operator.index(m) for m in seqlens]
+        except TypeError:
+            raise ValueError('extend: ids and seqlens must be sequences of ints') from None
+        if not ids or len(set(ids)) != len(ids):
+            raise ValueError(f'extend: ids must be distinct open clouds, at least one, got {ids[:16]}')
+        for c in ids:
+            self._known(c, 'extend')
+        if len(seqlens) != len(ids) or min(seqlens) < 1:
+            raise ValueError(f'extend: seqlens must hold one count >= 1 per listed cloud ({len(ids)}), got {seqlens[:16]}')
+        M = sum(seqlens)
+        n_cur = [self._len[c] + m for c, m in zip(ids, seqlens)]
+        short = [c for c, n in zip(ids, n_cur) if n < 2]
+        if short:
+            raise ValueError(f'extend: clouds {short[:16]} would have fewer than 2 nodes; the first call of a cloud needs at least '
+                             '2 nodes, as a forward does')
+        if _is_sparse(coors) or not torch.is_tensor(coors) or tuple(coors.shape) != (M, 3):
+            raise ValueError(f'extend: coors must be a dense [sum(seqlens), 3] = {(M, 3)} tensor, got '
+                             f'{tuple(coors.shape) if torch.is_tensor(coors) else type(coors).__name__}')
+        for t in (feats.values() if isinstance(feats, dict) else [feats]):
+            if not torch.is_tensor(t) or t.dim() < 1 or t.shape[0] != M or _is_sparse(t):
+                raise ValueError(f'extend: the features must be dense with sum(seqlens) = {M} rows, got '
+                                 f'{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}')
+        if model.has_edges and edges is None:
+            raise ValueError('extend: the model has edge features (edge_dim): pass edges for the new rows of every listed cloud')
+        if edges is not None and not model.has_edges:
+            raise ValueError('extend: edges given, but the model was built without edge_dim')
+        for name, per_cloud in (('edges', edges), ('neighbor_mask', neighbor_mask)):
+            if per_cloud is None:
+                continue
+            if not isinstance(per_cloud, (list, tuple)) or len(per_cloud) != len(ids):
+                raise ValueError(f'extend: {name} must be a list of {len(ids)} per-cloud tensors, got '
+                                 f'{len(per_cloud) if isinstance(per_cloud, (list, tuple)) else type(per_cloud).__name__}')
+            dims = 3 if name == 'edges' and not exists(model.edge_emb) else 2
+            for c, t, m, n in zip(ids, per_cloud, seqlens, n_cur):
+                if _is_sparse(t):
+                    raise ValueError(f'extend: {name} of cloud {c} is a sparse tensor; decoding takes dense rows')
+                if not torch.is_tensor(t) or t.dim() != dims or tuple(t.shape[:2]) != (m, n):
+                    want = f'[m, n_cur, edge_dim] = [{m}, {n}, edge_dim]' if dims == 3 else f'[m, n_cur] = [{m}, {n}]'
+                    raise ValueError(f'extend: {name} of cloud {c} must hold its new rows against all of its nodes so far, {want}, '
+                                     f'got {tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}')
+        if exists(model.pos_emb) and max(n_cur) > model.num_positions:
+            raise ValueError(f'extend: node {max(n_cur) - 1} is past num_positions = {model.num_positions}')
+        return ids, seqlens
+
+    # ---- one step ------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def extend(self, ids, seqlens, feats, coors, edges=None, neighbor_mask=None, return_type=None, return_pooled=False):
+        """Append seqlens[i] >= 1 nodes to each listed cloud ids[i] and return their outputs; clouds not listed do not move.
+        feats [M, dim_in] float, [M] tokens or {'d': [M, C, 2d+1]}; coors [M, 3]; M = sum(seqlens), rows in ids order.
+        edges: one [m_c, n_cur_c] token or [m_c, n_cur_c, edge_dim] float tensor per listed cloud; neighbor_mask: one bool
+        [m_c, n_cur_c] per listed cloud (the new rows against all of the cloud's nodes so far).  Returns what forward_packed
+        returns for those M rows: {'d': [M, C, 2d+1]} ('0': [M, C]), or one degree with return_type."""
+        ids, seqlens = self._check(ids, seqlens, feats, coors, edges, neighbor_mask, return_pooled)
+        out = self.model._checked(lambda: self._step(ids, seqlens, feats, coors, edges, neighbor_mask, return_type))
+        for c, m in zip(ids, seqlens):
+            self._len[c] += m
+        return out
+
+    def _grow(self, rows, n_cur, dev):
+        """Room for cache rows [0, rows) of n_cur nodes: each axis doubled when full, so a step never copies the whole prefix."""
+        S = self.S if rows <= self.S else max(rows, 2 * self.S)
+        cap = self.cap if n_cur <= self.cap else max(n_cur, 2 * self.cap, 16)
+        if self.coors is not None and (S, cap) == (self.S, self.cap):
+            return
+        keep = min(self.cap, max(self._len.values(), default=0))
+
+        def grown(t):
+            new = t.new_empty((S, cap) + tuple(t.shape[2:]))
+            new[:self.S, :keep] = t[:, :keep]
+            return new
+        if self.coors is None:
+            self.coors = torch.empty((0, 0, 3), dtype=torch.float32, device=dev)
+        self.coors = grown(self.coors)
+        self.stages = {name: ({d: grown(t) for d, t in feats.items()}, grown(nodemax)) for name, (feats, nodemax) in self.stages.items()}
+        self.S, self.cap = S, cap
+
+    def _step(self, ids, seqlens, feats, coors, edges, neighbor_mask, return_type):
+        """One extend (idempotent until the lengths move, so that a low-rank plan miss can run it again): (outputs, deferred
+        checks)."""
+        model = self.model
+        B, M = len(ids), sum(seqlens)
+        slots = [self._slot[c] for c in ids]
+        n_prev = [self._len[c] for c in ids]
+        n_cur = [p + m for p, m in zip(n_prev, seqlens)]
+        out_dtype = model._compute_dtype(coors)
+        if model.output_degrees == 1:
+            return_type = 0
+        dev = coors.device
+        # per new row: its position in its cloud, its cloud's cache row and where its pair row starts in the concatenated inputs
+        lens = torch.tensor(seqlens)
+        first = torch.repeat_interleave(lens.cumsum(0) - lens, lens)
+        local = torch.arange(M) - first
+        pair_off = torch.tensor([0] + [m * n for m, n in zip(seqlens, n_cur)][:-1]).cumsum(0)
+        rows = torch.stack((local + torch.repeat_interleave(torch.tensor(n_prev), lens), torch.repeat_interleave(torch.tensor(slots), lens),
+                            torch.repeat_interleave(pair_off, lens) + local * torch.repeat_interleave(torch.tensor(n_cur), lens)))
+        pos, slot_row, pair_row = rows.to(dev)
+        if isinstance(feats, dict):
+            feats = {d: v.unsqueeze(0) for d, v in feats.items()}
+        else:
+            feats = model._embed_tokens(feats.unsqueeze(0), pos)
+            feats = {'0': feats[..., None]}
+        feats = model._check_features(feats, coors)
+        self._grow(max(slots) + 1, max(n_cur), dev)
+        base = slot_row * self.cap                                          # the batch-1 view: node j of row s is s cap + j
+        dest = base + pos
+        self.coors.view(-1, 3).index_copy_(0, dest, coors.float())
+        ks = [model._num_neighbors(n, 0) for n in n_cur]
+        idx, nmask, rel_pos, rel_dist = ops.knn_rows_packed(
+            self.coors, slots, n_prev, seqlens, ks, model._valid_radius(), causal=True,
+            neighbor_mask=None if neighbor_mask is None else [t.to(dev) for t in neighbor_mask])
+        K = idx.shape[1]
+        local_idx = idx - base[:, None]
+        edge_values = None
+        if exists(edges):
+            edge_values = torch.cat([(t if exists(model.edge_emb) else t.float()).to(dev).reshape((-1,) + tuple(t.shape[2:]))
+                                     for t in edges])[pair_row[:, None] + local_idx]
+        e = model._edge_features(edge_values, None)
+        pos_emb = None
+        if exists(model.rotary_pos_emb):
+            pos_emb = model._rotary(pos.view(1, M), torch.cat((pos[:, None], local_idx), dim=1).view(1, M, 1 + K), max(n_cur),
+                                    rel_dist.view(1, M, K))
+        geom = Geometry(rel_pos[None], model.num_degrees - 1, deferred=[])
+        step = dict(dest=dest, rows=_StepRows(M), edge_info=(idx[None], nmask[None], None if e is None else e[None]),
+                    rel_dist=rel_dist[None], geom=geom)
+        return self._walk(feats, step, pos_emb, lambda v: v[0], out_dtype, return_type)
+
+    def _store(self, cache, rows, step):
+        """New row t goes to node n_prev_c + r of cache row slot_c, flat position dest[t] of the [S cap] view."""
+        cache.view((-1,) + tuple(cache.shape[2:])).index_copy_(0, step['dest'], rows)

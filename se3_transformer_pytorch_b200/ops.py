@@ -25,6 +25,7 @@ _SIGNATURES = {
     'se3_abi_version': (c_int, []),
     'se3_knn_fwd': (c_int, [c_void_p] * 7 + [c_int, c_int64, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
     'se3_knn_rows_fwd': (c_int, [c_void_p] * 3 + [c_int, c_int64, c_int64, c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 5),
+    'se3_knn_rows_packed_fwd': (c_int, [c_void_p] * 7 + [c_int, c_int64, c_int64, c_int, c_int, c_float, c_int] + [c_void_p] * 5),
     'se3_pair_lookup_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
@@ -195,6 +196,7 @@ def pair_lookup(rows, idx):
 
 
 MAX_CLOUD = 4097      # nodes per cloud of the shared-memory sort (n - 1 <= 4096 columns)
+KNN_MAX_K = 4096      # neighbours per node: the longest list the tiled search keeps next to its tile
 
 
 def pair_offsets(seqlens):
@@ -301,6 +303,66 @@ def knn_rows(coors, n, row0, m, k, valid_radius, *, node_mask=None, neighbor_mas
     with torch.cuda.device(dev), _timed('knn_rows', nbytes=12 * b * n + 25 * b * m * k):
         _check(lib().se3_knn_rows_fwd(_p(coors), _p(nm), _p(nbr), b, n, ld, row0, m, k, float(min(valid_radius, 3.0e38)),
                                       int(bool(causal)), _p(idx), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
+    return idx, mask.view(torch.bool), rel_pos, rel_dist
+
+
+def knn_rows_packed(coors, slots, n_prev, seqlens, k, valid_radius, *, neighbor_mask=None, causal=False):
+    """The neighbour search of the new rows of clouds of different lengths that grow on their own (PackedCausalDecoder): coors
+    [S, ld, 3] (contiguous float32) holds cloud c in row slots[c]; its seqlens[c] >= 1 new rows are nodes n_prev[c] + r,
+    searched over its first n_cur_c = n_prev[c] + seqlens[c] nodes for k[c] neighbours.  neighbor_mask: None, or a list with
+    one [seqlens[c], n_cur_c] bool mask (or None) per cloud.  Returns idx int64 [M, K] (M = sum(seqlens), K = max k_c; indices
+    slots[c] * ld + j in the [S * ld] view), mask bool [M, K], rel_pos [M, K, 3], rel_dist [M, K]: cloud c's rows are those of
+    knn_rows on that cloud alone in slots < k_c, and slots >= k_c repeat slot k_c - 1, masked.  The per-cloud descriptors are
+    checked here and uploaded in one copy; nothing is read back."""
+    if coors.dtype != torch.float32 or not coors.is_contiguous() or coors.dim() != 3 or coors.shape[2] != 3:
+        raise ValueError('knn_rows_packed: coors must be a contiguous float32 [S, ld, 3] tensor')
+    masks = list(neighbor_mask) if neighbor_mask is not None else None
+    _require_cuda(coors, *(masks or ()))
+    S, ld, _ = coors.shape
+    slots, n_prev, seqlens, k = ([int(v) for v in a] for a in (slots, n_prev, seqlens, k))
+    B = len(slots)
+    if B == 0 or not len(n_prev) == len(seqlens) == len(k) == B:
+        raise ValueError(f'knn_rows_packed: slots, n_prev, seqlens and k need one entry per cloud, got lengths '
+                         f'{[len(slots), len(n_prev), len(seqlens), len(k)]}')
+    n_cur = [p + m for p, m in zip(n_prev, seqlens)]
+    for c in range(B):
+        if not (0 <= slots[c] < S and n_prev[c] >= 0 and seqlens[c] >= 1 and 2 <= n_cur[c] <= ld and 1 <= k[c] <= n_cur[c] - 1):
+            raise ValueError(f'knn_rows_packed: cloud {c} needs 0 <= slot < {S}, n_prev >= 0, m >= 1, 2 <= n_prev + m <= ld = {ld} '
+                             f'and 1 <= k <= n_prev + m - 1 (got slot={slots[c]} n_prev={n_prev[c]} m={seqlens[c]} k={k[c]})')
+    K, M = max(k), sum(seqlens)
+    if K > KNN_MAX_K:
+        raise ValueError(f'knn_rows_packed: {K} neighbours exceed {KNN_MAX_K}, the longest list the tiled search keeps')
+    if M >= 2 ** 31:
+        raise ValueError(f'knn_rows_packed: {M} rows exceed the 1-D grid')
+    off, nbr = [-1] * B, None
+    if masks is not None:
+        if len(masks) != B:
+            raise ValueError(f'knn_rows_packed: neighbor_mask must have one entry per cloud ({B}), got {len(masks)}')
+        parts, at = [], 0
+        for c, t in enumerate(masks):
+            if t is None:
+                continue
+            if tuple(t.shape) != (seqlens[c], n_cur[c]):
+                raise ValueError(f'knn_rows_packed: neighbor_mask[{c}] must be [m, n_cur] = {(seqlens[c], n_cur[c])}, got {tuple(t.shape)}')
+            off[c] = at
+            at += t.numel()
+            parts.append(_u8(t).reshape(-1))
+        nbr = torch.cat(parts) if parts else None
+    cu = [0]
+    for m in seqlens:
+        cu.append(cu[-1] + m)
+    dev = coors.device
+    desc = torch.tensor(cu + slots + n_prev + k + off, dtype=torch.int64).to(dev)      # the one upload of the step's descriptors
+    cu_d, slot_d, prev_d, k_d, off_d = desc[:B + 1], desc[B + 1:2 * B + 1], desc[2 * B + 1:3 * B + 1], desc[3 * B + 1:4 * B + 1], desc[4 * B + 1:]
+    idx = torch.empty((M, K), dtype=torch.int64, device=dev)
+    mask = torch.empty((M, K), dtype=torch.uint8, device=dev)
+    rel_pos = torch.empty((M, K, 3), dtype=torch.float32, device=dev)
+    rel_dist = torch.empty((M, K), dtype=torch.float32, device=dev)
+    nbytes = 12 * sum(n_cur) + 25 * M * K + (0 if nbr is None else nbr.numel())
+    with torch.cuda.device(dev), _timed('knn_rows_packed', nbytes=nbytes):
+        _check(lib().se3_knn_rows_packed_fwd(_p(coors), _p(nbr), _p(cu_d), _p(slot_d), _p(prev_d), _p(k_d), _p(off_d), B, M, ld,
+                                             max(n_cur), K, float(min(valid_radius, 3.0e38)), int(bool(causal)), _p(idx), _p(mask),
+                                             _p(rel_pos), _p(rel_dist), _stream()))
     return idx, mask.view(torch.bool), rel_pos, rel_dist
 
 
