@@ -104,6 +104,20 @@ int se3_knn_rows_packed_fwd(const float* coors, const uint8_t* neighbor_mask, co
                             int64_t ld, int n_max, int K, float valid_radius, int causal, int64_t* out_idx, uint8_t* out_mask,
                             float* out_rel_pos, float* out_rel_dist, void* stream);
 
+/* The same search for clouds whose nodes sit in pages of page_size nodes of one pool (paged causal decoding).  pool
+ * [pages, page_size, 3]; cloud c's page ids are the int32 pages[table_off[c] ..], in node order, so its node j is pool row
+ * pages[table_off[c] + j / page_size] * page_size + j % page_size.  cu_rows, n_prev, k_per_cloud, pair_off, neighbor_mask and
+ * n_max are as in se3_knn_rows_packed_fwd.  out_idx [rows, K] gets the neighbours' pool rows and out_col [rows, K] their
+ * columns j in the cloud.  The caller guarantees what se3_knn_rows_packed_fwd's caller does, 0 <= table_off[c] < 2^31, and
+ * ceil(n_cur_c / page_size) valid page ids for each cloud; nothing is read back.  Row r of cloud c is bit for bit row
+ * n_prev[c] + r of se3_knn_rows_packed_fwd for the same cloud stored contiguously (out_col equal to its local indices, masks,
+ * rel_pos and rel_dist equal). */
+int se3_knn_rows_paged_fwd(const float* pool, const int* pages, const uint8_t* neighbor_mask, const int64_t* cu_rows,
+                           const int64_t* n_prev, const int64_t* k_per_cloud, const int64_t* pair_off, const int64_t* table_off,
+                           int num_clouds, int64_t rows, int page_size, int n_max, int K, float valid_radius, int causal,
+                           int64_t* out_idx, int64_t* out_col, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist,
+                           void* stream);
+
 /* Position of every neighbour in a sparse pair list (as in se3_pairs; batch_stride 0 when shared, else n): out[b,i,kk] = p with
  * cols[p] == idx[b,i,kk] inside row (b, i), or -1 if the row lacks that column.  idx, out: [b, n, k] int64.  The caller indexes
  * the list's values (edge tokens, edge features, hop counts) with a zero row appended for -1. */

@@ -83,12 +83,43 @@ struct CsrPairs {
   __device__ __forceinline__ bool bonded(int j) const { return adj && bit(bits + CSR_BITMAP_WORDS, j); }
 };
 
+// Where column j of a cloud keeps its coordinates.  Flat (const float* c): row j of the cloud's [n, 3] block, neighbour index
+// j_base + j.  PagedCoords: row pages[toff + j / P] P + j % P of a pool of pages of P nodes ([pages, P, 3]; pages[toff ..]: the
+// cloud's page ids in order); its neighbour index is the column j, which knn_rows_paged_kernel turns into the pool row.  Only the
+// address of a column differs: keys, ties and distances are the same, so a paged row is bit for bit the flat row of the same
+// cloud.  j / P is a multiply-high and a shift (page_divisor): with it, and with no pointer to the column output carried
+// through the search, the paged search fits 40 registers without spilling.
+struct PagedCoords {
+  const float* __restrict__ pool;
+  const int* __restrict__ pages;
+  int toff;
+  unsigned P, magic, shift;
+  __device__ __forceinline__ int64_t row(int j) const {
+    const unsigned q = (__umulhi((unsigned)j, magic) + (unsigned)j) >> shift;       // j / P for 0 <= j < 2^31
+    return (int64_t)pages[toff + q] * P + ((unsigned)j - q * P);
+  }
+};
+
+// magic, shift with (umulhi(j, magic) + j) >> shift = j / P for 0 <= j < 2^31 (Granlund and Montgomery, 1994): shift =
+// ceil(log2 P), magic = floor(2^32 (2^shift - P) / P) + 1.  The sum stays below 2^32 because umulhi(j, magic) < j < 2^31.
+static inline void page_divisor(unsigned P, unsigned& magic, unsigned& shift) {
+  shift = 0;
+  while ((1ull << shift) < P) ++shift;
+  magic = (unsigned)((((1ull << shift) - P) << 32) / P + 1);
+}
+__device__ __forceinline__ float coord(const float* __restrict__ c, int j, int d) { return c[j * 3 + d]; }
+__device__ __forceinline__ float coord(const PagedCoords& c, int j, int d) { return c.pool[c.row(j) * 3 + d]; }
+__device__ __forceinline__ void emit(const float* __restrict__, int64_t* __restrict__ out_idx, int r, int64_t j_base, int j) {
+  out_idx[r] = j_base + j;
+}
+__device__ __forceinline__ void emit(const PagedCoords&, int64_t* __restrict__ out_idx, int r, int64_t, int j) { out_idx[r] = j; }
+
 // keys[0, width) <- the keys of the self-removed columns [t0, t0 + width) of row i, ~0 past the last column.
 // key = (bits(modified distance) << 32) | column.  Distances are >= 0 so the IEEE bit pattern is order preserving; equal
 // distances order by column, which is the stable-argsort tie rule the oracle uses (torch.topk leaves ties unspecified).
 // Returns whether this thread wrote a key below `kth`.
-template <int THREADS, class Pairs>
-__device__ __forceinline__ bool knn_tile_keys(unsigned long long* keys, const float* __restrict__ c, int n, int i, float xi,
+template <int THREADS, class Pairs, class Coords>
+__device__ __forceinline__ bool knn_tile_keys(unsigned long long* keys, const Coords c, int n, int i, float xi,
                                               float yi, float zi, int t0, int width, const Pairs& pairs, int causal,
                                               unsigned long long kth) {
   bool below = false;
@@ -97,7 +128,7 @@ __device__ __forceinline__ bool knn_tile_keys(unsigned long long* keys, const fl
     unsigned long long key = ~0ull;
     if (jc < n - 1) {
       const int j = jc + (jc >= i);
-      const float dx = xi - c[j * 3 + 0], dy = yi - c[j * 3 + 1], dz = zi - c[j * 3 + 2];
+      const float dx = xi - coord(c, j, 0), dy = yi - coord(c, j, 1), dz = zi - coord(c, j, 2);
       float d = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
       if (pairs.excluded(j)) d = FLT_MAX;
       if (pairs.bonded(j)) d = 0.f;
@@ -127,18 +158,18 @@ __device__ __forceinline__ void knn_sort(unsigned long long* keys, int npad) {
   }
 }
 
-// The neighbour list of node i of one cloud of n nodes (c = that cloud's coordinates, [n, 3]); the same body for every cloud
+// The neighbour list of node i of one cloud of n nodes (c = where its coordinates are, see coord); the same body for every cloud
 // form and pair form of knn_kernel, so that all produce the same bits.  pairs:
 // row i of the cloud's pair masks (DensePairs or CsrPairs); node_mask: the cloud's [n] node mask (or NULL).  Writes slots
-// [0, K_out) of the row at out_*; slots r >= k are copies of slot k - 1 with mask 0, and indices are offset by j_base.
+// [0, K_out) of the row at out_*; slots r >= k are copies of slot k - 1 with mask 0, and indices are those of emit.
 // keys: npad = next_pow2(n - 1) keys of shared memory when n - 1 <= KNN_TILE (one sort of the whole row), otherwise
 // KNN_TILE + next_pow2(k) keys (tile, then running list).  Keys are unique, so every top-k order gives the bits of one full sort.
-template <int THREADS, class Pairs>
-__device__ __forceinline__ void knn_row(unsigned long long* keys, const float* __restrict__ c, int n, int i, int k, int npad,
+template <int THREADS, class Pairs, class Coords>
+__device__ __forceinline__ void knn_row(unsigned long long* keys, const Coords c, int n, int i, int k, int npad,
                                         Pairs pairs, const uint8_t* __restrict__ node_mask, float valid_radius, int causal, int K_out,
                                         int64_t j_base, int64_t* __restrict__ out_idx, uint8_t* __restrict__ out_mask,
                                         float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
-  const float xi = c[i * 3 + 0], yi = c[i * 3 + 1], zi = c[i * 3 + 2];
+  const float xi = coord(c, i, 0), yi = coord(c, i, 1), zi = coord(c, i, 2);
   const unsigned long long* best = keys;
   if (n - 1 <= KNN_TILE) {
     pairs.template stage<THREADS>(0, npad);
@@ -177,11 +208,11 @@ __device__ __forceinline__ void knn_row(unsigned long long* keys, const float* _
     const int jc = (int)(key & 0xffffffffu);
     const float dmod = __uint_as_float((unsigned)(key >> 32));
     const int j = jc + (jc >= i);
-    const float dx = xi - c[j * 3 + 0], dy = yi - c[j * 3 + 1], dz = zi - c[j * 3 + 2];
+    const float dx = xi - coord(c, j, 0), dy = yi - coord(c, j, 1), dz = zi - coord(c, j, 2);
     const float d = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
     bool m = r < k && dmod <= valid_radius;
     if (node_mask) m = m && mi && node_mask[j] != 0;
-    out_idx[r] = j_base + j;
+    emit(c, out_idx, r, j_base, j);
     out_mask[r] = m ? 1 : 0;
     out_rel_pos[r * 3 + 0] = dx;
     out_rel_pos[r * 3 + 1] = dy;
@@ -289,6 +320,38 @@ knn_rows_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ nod
   knn_row<THREADS>(keys, coors + c * ld * 3, n_c, i, k_c, knn_npad(n_c), DensePairs{row_mask, nullptr},
                    node_mask ? node_mask + c * ld : nullptr, valid_radius, causal, k, j_base, out_idx + o, out_mask + o,
                    out_rel_pos + o * 3, out_rel_dist + o);
+}
+
+// The ragged form of knn_rows_kernel for clouds kept in pages of P nodes of one pool, coors [pages, P, 3] (PagedCausalDecoder):
+// cloud c's page ids are pages[table_off[c] ..], and its node j is pool row pages[table_off[c] + j / P] P + j % P.  out_idx
+// gets that pool row, out_col the column j; everything else is as in knn_rows_kernel.  table_off < 2^31.
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS, 6)
+knn_rows_paged_kernel(const float* __restrict__ pool, const int* __restrict__ pages, const uint8_t* __restrict__ nbr,
+                      const int64_t* __restrict__ cu_rows, const int64_t* __restrict__ n_prev, const int64_t* __restrict__ k_per_cloud,
+                      const int64_t* __restrict__ pair_off, const int64_t* __restrict__ table_off, int num_clouds, unsigned P,
+                      unsigned magic, unsigned shift, int K, float valid_radius, int causal, int64_t* __restrict__ out_idx, int64_t* __restrict__ out_col,
+                      uint8_t* __restrict__ out_mask, float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
+  extern __shared__ unsigned long long keys[];
+  const int64_t t = blockIdx.x;
+  int lo = 0, hi = num_clouds - 1;                  // the last cloud with cu_rows[lo] <= t
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (cu_rows[mid] <= t) lo = mid; else hi = mid - 1;
+  }
+  const int64_t r = t - cu_rows[lo];
+  const int i = (int)(n_prev[lo] + r);
+  const int n_c = (int)(n_prev[lo] + cu_rows[lo + 1] - cu_rows[lo]);
+  const uint8_t* row_mask = nbr && pair_off[lo] >= 0 ? nbr + pair_off[lo] + r * n_c : nullptr;
+  const int64_t o = t * K;
+  const PagedCoords c{pool, pages, (int)table_off[lo], P, magic, shift};
+  knn_row<THREADS>(keys, c, n_c, i, (int)k_per_cloud[lo], knn_npad(n_c), DensePairs{row_mask, nullptr}, nullptr, valid_radius,
+                   causal, K, 0, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
+  for (int s = threadIdx.x; s < K; s += THREADS) {  // the slots this thread wrote in knn_row: columns -> pool rows
+    const int j = (int)out_idx[o + s];
+    out_col[o + s] = j;
+    out_idx[o + s] = c.row(j);
+  }
 }
 
 __global__ void gather_pairs_kernel(const float* __restrict__ pf, const int64_t* __restrict__ idx, int n, int k, int e,
@@ -451,6 +514,35 @@ extern "C" int se3_knn_rows_packed_fwd(const float* coors, const uint8_t* neighb
   SE3_REQUIRE(K >= 1 && K <= KNN_TILE, "se3_knn_rows_packed_fwd: K must be in [1, %d] (got %d)", KNN_TILE, K);
   return launch_knn_rows(coors, nullptr, neighbor_mask, cu_rows, slot, n_prev, k_per_cloud, pair_off, num_clouds, n_max, ld, 0, 1,
                          rows, K, valid_radius, causal, out_idx, out_mask, out_rel_pos, out_rel_dist, stream);
+}
+
+extern "C" int se3_knn_rows_paged_fwd(const float* pool, const int* pages, const uint8_t* neighbor_mask, const int64_t* cu_rows,
+                                      const int64_t* n_prev, const int64_t* k_per_cloud, const int64_t* pair_off,
+                                      const int64_t* table_off, int num_clouds, int64_t rows, int page_size, int n_max, int K,
+                                      float valid_radius, int causal, int64_t* out_idx, int64_t* out_col, uint8_t* out_mask,
+                                      float* out_rel_pos, float* out_rel_dist, void* stream) {
+  using namespace se3;
+  SE3_REQUIRE(pool && pages && cu_rows && n_prev && k_per_cloud && table_off && out_idx && out_col && out_mask && out_rel_pos &&
+              out_rel_dist, "se3_knn_rows_paged_fwd: null pointer");
+  SE3_REQUIRE(!neighbor_mask || pair_off, "se3_knn_rows_paged_fwd: a neighbour mask needs pair_off");
+  SE3_REQUIRE(num_clouds > 0 && rows >= num_clouds && rows < (1ll << 31),
+              "se3_knn_rows_paged_fwd: need 0 < num_clouds <= rows < 2^31 (got %d clouds, %lld rows)", num_clouds, (long long)rows);
+  SE3_REQUIRE(page_size >= 1, "se3_knn_rows_paged_fwd: page_size must be >= 1 (got %d)", page_size);
+  SE3_REQUIRE(n_max > 1, "se3_knn_rows_paged_fwd: need n_max > 1 (got %d)", n_max);
+  SE3_REQUIRE(K >= 1 && K <= KNN_TILE, "se3_knn_rows_paged_fwd: K must be in [1, %d] (got %d)", KNN_TILE, K);
+  constexpr int THREADS = 256;
+  const int key_words = n_max - 1 > KNN_TILE ? KNN_TILE + next_pow2(K) : knn_npad(n_max);
+  const size_t smem = (size_t)key_words * sizeof(unsigned long long);
+  unsigned magic, shift;
+  page_divisor((unsigned)page_size, magic, shift);
+  auto kernel = knn_rows_paged_kernel<THREADS>;
+  if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)rows, THREADS, smem, as_stream(stream)>>>(pool, pages, neighbor_mask, cu_rows, n_prev, k_per_cloud, pair_off,
+                                                               table_off, num_clouds, (unsigned)page_size, magic, shift, K,
+                                                               valid_radius, causal, out_idx, out_col, out_mask, out_rel_pos,
+                                                               out_rel_dist);
+  SE3_LAUNCH_OK();
+  return SE3_OK;
 }
 
 extern "C" int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx,

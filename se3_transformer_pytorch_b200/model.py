@@ -8,6 +8,7 @@ libse3b200.so through `ops`; the cheap glue around it (embeddings, LinearSE3 GEM
 
 Forward only: everything runs under torch.no_grad().  CUDA only: there is no CPU fallback.
 """
+import numbers
 import operator
 from math import sqrt
 from typing import NamedTuple
@@ -1393,10 +1394,17 @@ class SE3Transformer(nn.Module):
         doing the edge work of its new nodes only."""
         return CausalDecoder(self, batch_size)
 
-    def packed_decoder(self):
+    def packed_decoder(self, page_size=None, max_nodes=None):
         """An empty PackedCausalDecoder of this causal model: clouds of different lengths decoded together, each opened, extended,
-        truncated, forked and closed on its own, every step carrying the new nodes of any subset of them."""
-        return PackedCausalDecoder(self)
+        truncated, forked and closed on its own, every step carrying the new nodes of any subset of them.  With an integer
+        page_size >= 1, a PagedCausalDecoder instead, the same decoder with its cache in pages of page_size nodes: memory follows
+        the nodes decoded and forks share their prefix; max_nodes (pages for that many nodes, reserved at the first step) caps
+        its pool, which otherwise doubles when full."""
+        if page_size is None:
+            if max_nodes is not None:
+                raise ValueError('packed_decoder: max_nodes caps the pages of a paged cache; give a page_size too')
+            return PackedCausalDecoder(self)
+        return PagedCausalDecoder(self, page_size, max_nodes)
 
     # ---- forward ----------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -2265,11 +2273,11 @@ class PackedCausalDecoder(_DecoderStages):
         return self._len[cloud]
 
     def open_ids(self):
-        return sorted(self._slot)
+        return sorted(self._len)
 
     def _known(self, cloud, api):
         try:
-            if operator.index(cloud) in self._slot:
+            if operator.index(cloud) in self._len:
                 return
         except TypeError:
             pass
@@ -2335,10 +2343,15 @@ class PackedCausalDecoder(_DecoderStages):
         [m_c, n_cur_c] per listed cloud (the new rows against all of the cloud's nodes so far).  Returns what forward_packed
         returns for those M rows: {'d': [M, C, 2d+1]} ('0': [M, C]), or one degree with return_type."""
         ids, seqlens = self._check(ids, seqlens, feats, coors, edges, neighbor_mask, return_pooled)
+        self._reserve(ids, seqlens, coors)
         out = self.model._checked(lambda: self._step(ids, seqlens, feats, coors, edges, neighbor_mask, return_type))
         for c, m in zip(ids, seqlens):
             self._len[c] += m
         return out
+
+    def _reserve(self, ids, seqlens, coors):
+        """Room in the cache for the step, made once before its body (which a low-rank plan miss runs again).  The rows of this
+        cache grow inside the body (_search), which is idempotent."""
 
     def _grow(self, rows, n_cur, dev):
         """Room for cache rows [0, rows) of n_cur nodes: each axis doubled when full, so a step never copies the whole prefix."""
@@ -2363,37 +2376,31 @@ class PackedCausalDecoder(_DecoderStages):
         checks)."""
         model = self.model
         B, M = len(ids), sum(seqlens)
-        slots = [self._slot[c] for c in ids]
         n_prev = [self._len[c] for c in ids]
         n_cur = [p + m for p, m in zip(n_prev, seqlens)]
         out_dtype = model._compute_dtype(coors)
         if model.output_degrees == 1:
             return_type = 0
         dev = coors.device
-        # per new row: its position in its cloud, its cloud's cache row and where its pair row starts in the concatenated inputs
+        # per new row: its position in its cloud, where it goes (_where) and where its pair row starts in the concatenated inputs
         lens = torch.tensor(seqlens)
         first = torch.repeat_interleave(lens.cumsum(0) - lens, lens)
         local = torch.arange(M) - first
         pair_off = torch.tensor([0] + [m * n for m, n in zip(seqlens, n_cur)][:-1]).cumsum(0)
-        rows = torch.stack((local + torch.repeat_interleave(torch.tensor(n_prev), lens), torch.repeat_interleave(torch.tensor(slots), lens),
+        pos = local + torch.repeat_interleave(torch.tensor(n_prev), lens)
+        rows = torch.stack((pos, self._where(ids, lens, pos),
                             torch.repeat_interleave(pair_off, lens) + local * torch.repeat_interleave(torch.tensor(n_cur), lens)))
-        pos, slot_row, pair_row = rows.to(dev)
+        pos, where, pair_row = rows.to(dev)
         if isinstance(feats, dict):
             feats = {d: v.unsqueeze(0) for d, v in feats.items()}
         else:
             feats = model._embed_tokens(feats.unsqueeze(0), pos)
             feats = {'0': feats[..., None]}
         feats = model._check_features(feats, coors)
-        self._grow(max(slots) + 1, max(n_cur), dev)
-        base = slot_row * self.cap                                          # the batch-1 view: node j of row s is s cap + j
-        dest = base + pos
-        self.coors.view(-1, 3).index_copy_(0, dest, coors.float())
         ks = [model._num_neighbors(n, 0) for n in n_cur]
-        idx, nmask, rel_pos, rel_dist = ops.knn_rows_packed(
-            self.coors, slots, n_prev, seqlens, ks, model._valid_radius(), causal=True,
-            neighbor_mask=None if neighbor_mask is None else [t.to(dev) for t in neighbor_mask])
+        dest, idx, local_idx, nmask, rel_pos, rel_dist = self._search(
+            ids, n_prev, seqlens, ks, pos, where, coors, None if neighbor_mask is None else [t.to(dev) for t in neighbor_mask])
         K = idx.shape[1]
-        local_idx = idx - base[:, None]
         edge_values = None
         if exists(edges):
             edge_values = torch.cat([(t if exists(model.edge_emb) else t.float()).to(dev).reshape((-1,) + tuple(t.shape[2:]))
@@ -2408,6 +2415,239 @@ class PackedCausalDecoder(_DecoderStages):
                     rel_dist=rel_dist[None], geom=geom)
         return self._walk(feats, step, pos_emb, lambda v: v[0], out_dtype, return_type)
 
+    def _where(self, ids, lens, pos):
+        """What _search needs to place each new row (pos: its node in its cloud), host int64 [M]: its cloud's cache row."""
+        return torch.repeat_interleave(torch.tensor([self._slot[c] for c in ids]), lens)
+
+    def _search(self, ids, n_prev, seqlens, ks, pos, where, coors, neighbor_mask):
+        """Store the step's coordinates and search its new rows' neighbours: (dest [M], the new rows' positions in the flat cache;
+        idx [M, K], the neighbours' positions there; their columns in their clouds [M, K]; mask, rel_pos, rel_dist)."""
+        slots = [self._slot[c] for c in ids]
+        self._grow(max(slots) + 1, max(p + m for p, m in zip(n_prev, seqlens)), coors.device)
+        base = where * self.cap                                             # the batch-1 view: node j of row s is s cap + j
+        dest = base + pos
+        self.coors.view(-1, 3).index_copy_(0, dest, coors.float())
+        idx, nmask, rel_pos, rel_dist = ops.knn_rows_packed(self.coors, slots, n_prev, seqlens, ks, self.model._valid_radius(),
+                                                            causal=True, neighbor_mask=neighbor_mask)
+        return dest, idx, idx - base[:, None], nmask, rel_pos, rel_dist
+
     def _store(self, cache, rows, step):
-        """New row t goes to node n_prev_c + r of cache row slot_c, flat position dest[t] of the [S cap] view."""
+        """New row t goes to flat position dest[t] of the cache (node n_prev_c + r of cache row slot_c)."""
         cache.view((-1,) + tuple(cache.shape[2:])).index_copy_(0, step['dest'], rows)
+
+
+class DecoderCacheFull(RuntimeError):
+    """A step of a PagedCausalDecoder with max_nodes needs more pages than its pool has free.  Raised before any device work,
+    with the decoder unchanged: close, truncate or pre-empt clouds and send the step again."""
+
+
+class StepPages(NamedTuple):
+    """What a step needs from PageTables.plan: the pool size after it, the copy-on-write pages (cloud, index in its table, rows
+    to copy) and the fresh pages each listed cloud appends."""
+    reserved: int
+    cow: list
+    fresh: list
+
+
+class PageTables:
+    """The page bookkeeping of a PagedCausalDecoder, on the host (it holds no tensors): each cloud's block table, the ids of the
+    pages that hold its nodes [0, P), [P, 2P), ...; one reference count per page; and a free list.  The pool has `reserved`
+    pages on the device; a page that no table references is free, and allocations take freed pages first (the most recent
+    first).  A cloud of n nodes has at least ceil(n / P) pages: more only after a step failed once its pages were taken."""
+
+    def __init__(self, page_size, max_pages=None):
+        self.P, self.max_pages = page_size, max_pages
+        self.reserved = 0
+        self.refs = []                            # page id -> number of tables that hold it
+        self.free = []                            # unreferenced page ids, taken from the end
+        self.tables = {}                          # cloud -> page ids
+
+    def pages_in_use(self):
+        return self.reserved - len(self.free)
+
+    def open(self, cloud):
+        self.tables[cloud] = []
+
+    def close(self, cloud):
+        self._drop(self.tables.pop(cloud))
+
+    def truncate(self, cloud, n):
+        """Drop the cloud's pages past its first n nodes."""
+        table = self.tables[cloud]
+        keep = -(-n // self.P)
+        self._drop(table[keep:])
+        del table[keep:]
+
+    def fork(self, cloud, new, n):
+        """new shares the pages of cloud's first n nodes."""
+        table = self.tables[cloud][:-(-n // self.P)]
+        for p in table:
+            self.refs[p] += 1
+        self.tables[new] = list(table)
+
+    def _drop(self, pages):
+        for p in pages:
+            self.refs[p] -= 1
+            if not self.refs[p]:
+                self.free.append(p)
+
+    def plan(self, ids, n_prev, seqlens):
+        """The pages a step that appends seqlens[i] nodes to cloud ids[i] of n_prev[i] nodes needs (StepPages), without changing
+        anything.  A step writes nodes >= n_prev only, so the one page of a cloud that it may write while another cloud holds it
+        is the page of node n_prev, when n_prev is not a page boundary: that page is copied on write, its first n_prev % P rows.
+        Clouds are planned in order, so of siblings that write one shared page in the same step the last writes it in place.
+        Raises DecoderCacheFull if a capped pool has too few free pages."""
+        P = self.P
+        refs, cow, fresh = {}, [], []
+        for c, p, m in zip(ids, n_prev, seqlens):
+            table = self.tables[c]
+            if p % P:
+                page = table[p // P]
+                r = refs.get(page, self.refs[page])
+                if r > 1:
+                    cow.append((c, p // P, p % P))
+                    refs[page] = r - 1
+            fresh.append(max(0, -(-(p + m) // P) - len(table)))
+        need = len(cow) + sum(fresh)
+        if self.max_pages is not None:
+            if need > len(self.free) + self.max_pages - self.reserved:
+                raise DecoderCacheFull(f'extend: the step needs {need} free pages of {P} nodes and the pool has '
+                                       f'{len(self.free) + self.max_pages - self.reserved} of {self.max_pages} (max_nodes); close, '
+                                       'truncate or pre-empt clouds and retry')
+            return StepPages(self.max_pages, cow, fresh)
+        short = need - len(self.free)
+        return StepPages(self.reserved if short <= 0 else max(2 * self.reserved, self.reserved + short), cow, fresh)
+
+    def commit(self, plan, ids):
+        """Take the planned pages: grow the pool to plan.reserved, give each copy-on-write cloud a fresh page in place of the
+        shared one and append fresh pages.  Returns the copies [(old page, new page, rows)] that the caller makes on the device."""
+        if plan.reserved > self.reserved:
+            self.free[:0] = range(plan.reserved - 1, self.reserved - 1, -1)      # new pages after the freed ones, lowest first
+            self.refs += [0] * (plan.reserved - self.reserved)
+            self.reserved = plan.reserved
+        copies = []
+        for c, at, rows in plan.cow:
+            old, new = self.tables[c][at], self._take()
+            self.tables[c][at] = new
+            self.refs[old] -= 1                   # still held by the cloud it was shared with
+            copies.append((old, new, rows))
+        for c, f in zip(ids, plan.fresh):
+            self.tables[c] += [self._take() for _ in range(f)]
+        return copies
+
+    def _take(self):
+        p = self.free.pop()
+        self.refs[p] = 1
+        return p
+
+
+class PagedCausalDecoder(PackedCausalDecoder):
+    """PackedCausalDecoder with its cache in pages of page_size nodes (SE3Transformer.packed_decoder(page_size=...)): the same
+    open, extend, truncate, fork, close, length and open_ids, with the same results, refusals and messages, while memory
+    follows the nodes decoded and forked clouds share their prefix.
+
+    Every stage is [pages, P, C, 2d+1], with node maxima [pages, P] and coordinates [pages, P, 3], and each cloud has a block
+    table on the host (PageTables): node j of cloud c is row j % P of page table_c[j // P].  The neighbour search reads
+    coordinates through the tables and returns pool rows, which every later kernel reads in the flat [1, pages P, ...] view,
+    as it reads cache rows of the packed decoder; rows are therefore bit for bit the packed decoder's.  fork shares every page
+    of the parent and does no device work; truncate and close drop references, and a page nobody references is reused.  A
+    step writes nodes >= n_prev only, so before it runs, a page it would write while another cloud holds it is copied
+    (PageTables.plan).  The pool doubles when it runs out of pages, or, with max_nodes, is fixed at ceil(max_nodes / P) pages
+    and a step that does not fit raises DecoderCacheFull before any device work, leaving the decoder unchanged."""
+
+    def __init__(self, model, page_size, max_nodes=None):
+        _DecoderStages.__init__(self, model, 'packed_decoder')
+        if isinstance(page_size, bool) or not isinstance(page_size, numbers.Integral) or page_size < 1:
+            raise ValueError(f'packed_decoder: page_size must be None or an integer >= 1, got {page_size!r}')
+        if max_nodes is not None and (isinstance(max_nodes, bool) or not isinstance(max_nodes, numbers.Integral) or max_nodes < 1):
+            raise ValueError(f'packed_decoder: max_nodes must be None or an integer >= 1, got {max_nodes!r}')
+        self.page_size = int(page_size)
+        self.max_nodes = None if max_nodes is None else int(max_nodes)
+        self._book = PageTables(self.page_size, None if max_nodes is None else -(-self.max_nodes // self.page_size))
+        self._next_id = 0
+        self._len = {}                            # open cloud id -> number of nodes
+
+    def pages_in_use(self):
+        """Distinct pages that open clouds reference."""
+        return self._book.pages_in_use()
+
+    def pages_reserved(self):
+        """Pages allocated on the device."""
+        return self._book.reserved
+
+    # ---- lifecycle -----------------------------------------------------------------------------------------
+    def open(self, count=1):
+        """count new empty clouds; returns their ids, increasing integers that are never reused."""
+        if operator.index(count) < 1:
+            raise ValueError(f'open: count must be >= 1, got {count}')
+        ids = list(range(self._next_id, self._next_id + int(count)))
+        for c in ids:
+            self._len[c] = 0
+            self._book.open(c)
+        self._next_id += int(count)
+        return ids
+
+    def close(self, cloud):
+        """Forget a cloud; the pages only it held are free for the next allocation."""
+        self._known(cloud, 'close')
+        del self._len[cloud]
+        self._book.close(cloud)
+
+    def truncate(self, cloud, n):
+        """Rewind a cloud to its first n nodes (0 <= n <= length) and drop its pages past them."""
+        super().truncate(cloud, n)
+        self._book.truncate(cloud, self._len[cloud])
+
+    def fork(self, cloud):
+        """A new cloud whose nodes so far are `cloud`'s, sharing its pages (no device work, nothing allocated); returns its id."""
+        self._known(cloud, 'fork')
+        new = self.open()[0]
+        self._len[new] = self._len[cloud]
+        self._book.fork(cloud, new, self._len[cloud])
+        return new
+
+    # ---- one step ------------------------------------------------------------------------------------------
+    def _reserve(self, ids, seqlens, coors):
+        """Every page of the step, and its copies on write, before its body: the body must stay idempotent."""
+        plan = self._book.plan(ids, [self._len[c] for c in ids], seqlens)
+        ops._require_cuda(coors)
+        self._grow(plan.reserved, coors.device)
+        copies = self._book.commit(plan, ids)
+        if copies:
+            P = self.page_size
+            rows = torch.tensor([[old * P + r for old, _, n in copies for r in range(n)],
+                                 [new * P + r for _, new, n in copies for r in range(n)]]).to(coors.device)
+            for t in self._tensors():
+                flat = t.view((-1,) + tuple(t.shape[2:]))
+                flat.index_copy_(0, rows[1], flat.index_select(0, rows[0]))
+
+    def _tensors(self):
+        return [self.coors] + [t for feats, nodemax in self.stages.values() for t in (*feats.values(), nodemax)]
+
+    def _grow(self, pages, dev):
+        """A pool of `pages` pages, the old pool copied to its first pages (page ids do not change)."""
+        if self.coors is not None and pages <= self.coors.shape[0]:
+            return
+
+        def grown(t):
+            new = t.new_empty((pages,) + tuple(t.shape[1:]))
+            new[:t.shape[0]] = t
+            return new
+        if self.coors is None:
+            self.coors = torch.empty((0, self.page_size, 3), dtype=torch.float32, device=dev)
+        self.coors = grown(self.coors)
+        self.stages = {name: ({d: grown(t) for d, t in feats.items()}, grown(nodemax)) for name, (feats, nodemax) in self.stages.items()}
+
+    def _where(self, ids, lens, pos):
+        """Each new row's pool row, table_c[pos // P] P + pos % P."""
+        P, tables = self.page_size, [self._book.tables[c] for c in ids]
+        start = torch.tensor([0] + [len(t) for t in tables][:-1]).cumsum(0)
+        flat = torch.tensor([p for t in tables for p in t], dtype=torch.int64)
+        return flat[torch.repeat_interleave(start, lens) + pos // P] * P + pos % P
+
+    def _search(self, ids, n_prev, seqlens, ks, pos, where, coors, neighbor_mask):
+        self.coors.view(-1, 3).index_copy_(0, where, coors.float())
+        idx, col, nmask, rel_pos, rel_dist = ops.knn_rows_paged(self.coors, [self._book.tables[c] for c in ids], n_prev, seqlens,
+                                                                ks, self.model._valid_radius(), causal=True,
+                                                                neighbor_mask=neighbor_mask)
+        return where, idx, col, nmask, rel_pos, rel_dist

@@ -26,6 +26,7 @@ _SIGNATURES = {
     'se3_knn_fwd': (c_int, [c_void_p] * 7 + [c_int, c_int64, c_int, c_float, c_int] + [c_void_p] * 4 + [c_void_p]),
     'se3_knn_rows_fwd': (c_int, [c_void_p] * 3 + [c_int, c_int64, c_int64, c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 5),
     'se3_knn_rows_packed_fwd': (c_int, [c_void_p] * 7 + [c_int, c_int64, c_int64, c_int, c_int, c_float, c_int] + [c_void_p] * 5),
+    'se3_knn_rows_paged_fwd': (c_int, [c_void_p] * 8 + [c_int, c_int64, c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 6),
     'se3_pair_lookup_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
@@ -334,20 +335,7 @@ def knn_rows_packed(coors, slots, n_prev, seqlens, k, valid_radius, *, neighbor_
         raise ValueError(f'knn_rows_packed: {K} neighbours exceed {KNN_MAX_K}, the longest list the tiled search keeps')
     if M >= 2 ** 31:
         raise ValueError(f'knn_rows_packed: {M} rows exceed the 1-D grid')
-    off, nbr = [-1] * B, None
-    if masks is not None:
-        if len(masks) != B:
-            raise ValueError(f'knn_rows_packed: neighbor_mask must have one entry per cloud ({B}), got {len(masks)}')
-        parts, at = [], 0
-        for c, t in enumerate(masks):
-            if t is None:
-                continue
-            if tuple(t.shape) != (seqlens[c], n_cur[c]):
-                raise ValueError(f'knn_rows_packed: neighbor_mask[{c}] must be [m, n_cur] = {(seqlens[c], n_cur[c])}, got {tuple(t.shape)}')
-            off[c] = at
-            at += t.numel()
-            parts.append(_u8(t).reshape(-1))
-        nbr = torch.cat(parts) if parts else None
+    off, nbr = _row_masks('knn_rows_packed', masks, seqlens, n_cur)
     cu = [0]
     for m in seqlens:
         cu.append(cu[-1] + m)
@@ -364,6 +352,88 @@ def knn_rows_packed(coors, slots, n_prev, seqlens, k, valid_radius, *, neighbor_
                                              max(n_cur), K, float(min(valid_radius, 3.0e38)), int(bool(causal)), _p(idx), _p(mask),
                                              _p(rel_pos), _p(rel_dist), _stream()))
     return idx, mask.view(torch.bool), rel_pos, rel_dist
+
+
+def _row_masks(api, masks, seqlens, n_cur):
+    """The new rows' neighbour masks of a ragged row search (None, or one [m_c, n_cur_c] bool mask or None per cloud) end to end
+    as uint8: (per-cloud offsets, -1 for none, and the buffer or None)."""
+    B = len(seqlens)
+    off, nbr = [-1] * B, None
+    if masks is not None:
+        if len(masks) != B:
+            raise ValueError(f'{api}: neighbor_mask must have one entry per cloud ({B}), got {len(masks)}')
+        parts, at = [], 0
+        for c, t in enumerate(masks):
+            if t is None:
+                continue
+            if tuple(t.shape) != (seqlens[c], n_cur[c]):
+                raise ValueError(f'{api}: neighbor_mask[{c}] must be [m, n_cur] = {(seqlens[c], n_cur[c])}, got {tuple(t.shape)}')
+            off[c] = at
+            at += t.numel()
+            parts.append(_u8(t).reshape(-1))
+        nbr = torch.cat(parts) if parts else None
+    return off, nbr
+
+
+def knn_rows_paged(pool, tables, n_prev, seqlens, k, valid_radius, *, neighbor_mask=None, causal=False):
+    """The neighbour search of the new rows of clouds kept in pages (PagedCausalDecoder): pool [pages, P, 3] (contiguous float32)
+    holds node j of cloud c at row tables[c][j // P] * P + j % P of its [pages * P, 3] view; tables[c] lists at least
+    ceil(n_cur_c / P) page ids.  n_prev, seqlens, k and neighbor_mask are as in knn_rows_packed.  Returns idx int64 [M, K] (the
+    neighbours' pool rows), col int64 [M, K] (their columns j in the cloud), mask bool [M, K], rel_pos [M, K, 3] and rel_dist
+    [M, K]: cloud c's rows are knn_rows_packed's for the same cloud stored contiguously, with col its local indices.  The
+    descriptors and page lists are checked here and uploaded in one copy; nothing is read back."""
+    if pool.dtype != torch.float32 or not pool.is_contiguous() or pool.dim() != 3 or pool.shape[2] != 3:
+        raise ValueError('knn_rows_paged: pool must be a contiguous float32 [pages, page_size, 3] tensor')
+    masks = list(neighbor_mask) if neighbor_mask is not None else None
+    _require_cuda(pool, *(masks or ()))
+    pages, P, _ = pool.shape
+    tables = [[int(v) for v in t] for t in tables]
+    n_prev, seqlens, k = ([int(v) for v in a] for a in (n_prev, seqlens, k))
+    B = len(tables)
+    if B == 0 or not len(n_prev) == len(seqlens) == len(k) == B:
+        raise ValueError(f'knn_rows_paged: tables, n_prev, seqlens and k need one entry per cloud, got lengths '
+                         f'{[len(tables), len(n_prev), len(seqlens), len(k)]}')
+    n_cur = [p + m for p, m in zip(n_prev, seqlens)]
+    for c in range(B):
+        if not (n_prev[c] >= 0 and seqlens[c] >= 1 and 2 <= n_cur[c] < 2 ** 31 and 1 <= k[c] <= n_cur[c] - 1):
+            raise ValueError(f'knn_rows_paged: cloud {c} needs n_prev >= 0, m >= 1, 2 <= n_prev + m < 2^31 and '
+                             f'1 <= k <= n_prev + m - 1 (got n_prev={n_prev[c]} m={seqlens[c]} k={k[c]})')
+        need = -(-n_cur[c] // P)
+        if len(tables[c]) < need or not all(0 <= p < pages for p in tables[c][:need]):
+            raise ValueError(f'knn_rows_paged: cloud {c} needs {need} page ids in [0, {pages}) for its {n_cur[c]} nodes, got '
+                             f'{tables[c][:need]}')
+    K, M = max(k), sum(seqlens)
+    if K > KNN_MAX_K:
+        raise ValueError(f'knn_rows_paged: {K} neighbours exceed {KNN_MAX_K}, the longest list the tiled search keeps')
+    if M >= 2 ** 31:
+        raise ValueError(f'knn_rows_paged: {M} rows exceed the 1-D grid')
+    off, nbr = _row_masks('knn_rows_paged', masks, seqlens, n_cur)
+    cu, toff = [0], [0]
+    for m, t in zip(seqlens, tables):
+        cu.append(cu[-1] + m)
+        toff.append(toff[-1] + len(t))
+    if toff[-1] >= 2 ** 31:
+        raise ValueError(f'knn_rows_paged: {toff[-1]} page ids exceed 2^31')
+    # the one upload of the step: int64 descriptors [cu_rows | n_prev | k | pair_off | table_off], then the int32 page ids
+    nd = 5 * B + 1
+    host = torch.empty(2 * nd + toff[-1], dtype=torch.int32)
+    host[:2 * nd].view(torch.int64).copy_(torch.tensor(cu + n_prev + k + off + toff[:-1], dtype=torch.int64))
+    host[2 * nd:] = torch.tensor([p for t in tables for p in t], dtype=torch.int32)
+    dev = pool.device
+    buf = host.to(dev)
+    desc, page_ids = buf[:2 * nd].view(torch.int64), buf[2 * nd:]
+    cu_d, prev_d, k_d, off_d, toff_d = desc[:B + 1], desc[B + 1:2 * B + 1], desc[2 * B + 1:3 * B + 1], desc[3 * B + 1:4 * B + 1], desc[4 * B + 1:]
+    idx = torch.empty((M, K), dtype=torch.int64, device=dev)
+    col = torch.empty((M, K), dtype=torch.int64, device=dev)
+    mask = torch.empty((M, K), dtype=torch.uint8, device=dev)
+    rel_pos = torch.empty((M, K, 3), dtype=torch.float32, device=dev)
+    rel_dist = torch.empty((M, K), dtype=torch.float32, device=dev)
+    nbytes = 16 * sum(n_cur) + 33 * M * K + (0 if nbr is None else nbr.numel())
+    with torch.cuda.device(dev), _timed('knn_rows_paged', nbytes=nbytes):
+        _check(lib().se3_knn_rows_paged_fwd(_p(pool), _p(page_ids), _p(nbr), _p(cu_d), _p(prev_d), _p(k_d), _p(off_d), _p(toff_d),
+                                            B, M, P, max(n_cur), K, float(min(valid_radius, 3.0e38)), int(bool(causal)), _p(idx),
+                                            _p(col), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
+    return idx, col, mask.view(torch.bool), rel_pos, rel_dist
 
 
 def gather_pairs(pair_feat, idx):
