@@ -638,7 +638,7 @@ def fold_basis(S, basis_pair, E, Co, P, Q, F, out, accumulate, component_major=F
 
 def rotate_back(parts, D, E, Co, lo, out):
     """out [E,Co,2lo+1] = D_lo(e) out'(e): parts[0] [E,Co] (m = 0), parts[m] [E,Co,2] (components +m, -m) or None."""
-    _require_cuda(D, out)
+    _require_cuda(D, out, *parts)
     ptrs = [(_p(t) if t is not None else None) for t in (list(parts) + [None] * 4)[:4]]
     P = 2 * lo + 1
     nbytes = 4 * (2 * E * Co * P + E * P * P)

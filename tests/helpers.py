@@ -99,10 +99,105 @@ def decode_operand_image(img_u8):
     return out[:, 0], out[:, 1]
 
 
-def decode_T(T, n_tiles, Ci, F, P):
-    """tile layout [tile][ifb][4][PH][128][4] -> [n_tiles*128, Ci*F, P]."""
+def decode_T(T, n_tiles, Ci, F, P, padded=False):
+    """tile layout [tile][ifb][4][PH][128][4] -> [n_tiles*128, Ci*F, P] (padded: [n_tiles*128, 4*ifb, 4*PH], the padding slots
+    of the layout included)."""
     nifb = (Ci * F + 3) // 4
     ph = (P + 3) // 4
     t = T[: n_tiles * nifb * 4 * ph * 128 * 4].reshape(n_tiles, nifb * 4, ph, 128, 4)
     t = t.transpose(0, 3, 1, 2, 4).reshape(n_tiles * 128, nifb * 4, ph * 4)
-    return t[:, : Ci * F, :P]
+    return t if padded else t[:, : Ci * F, :P]
+
+
+# ---- the production GEMM (csrc/zgemm.cu) on random operands, and its float64 restatement ----
+def x_tile_layout(xp):
+    """x' [E, Ci, ncomp] -> zgemm's X layout [tiles][Ci][ncomp][128] (zero rows past E)."""
+    import torch
+    E, Ci, nc = xp.shape
+    tiles = (E + 127) // 128
+    buf = torch.zeros(tiles * 128, Ci, nc, dtype=torch.float32, device=xp.device)
+    buf[:E] = xp
+    return buf.reshape(tiles, 128, Ci, nc).permute(0, 2, 3, 1).contiguous().reshape(-1)
+
+
+def zgemm_reference(mode, segs, Co):
+    """float64: segs = [(U [E,Kp], Fp [Co*Ci*F, Kp], x' [E,Ci,ncomp], cplus, cminus)] -> out [E, mode, Co]."""
+    import torch
+    outs = None
+    mode = min(mode, 2)                                              # mode 3 computes what mode 2 computes (Gauss form)
+    for U, Fp, xp, cp, cm in segs:
+        E, Ci = xp.shape[0], xp.shape[1]
+        Fv = Fp.double().reshape(Co, Ci, mode, -1)
+        Ud = U.double()[:, :Fv.shape[-1]]
+        w = torch.einsum('ek,oifk->eoif', Ud, Fv)                     # the radial weights of this segment
+        xd = xp.double()
+        if mode == 1:
+            o = torch.einsum('eoi,ei->eo', w[..., 0], xd[:, :, cp])[:, None]
+        else:
+            a, b = w[..., 0], w[..., 1]
+            op = torch.einsum('eoi,ei->eo', a, xd[:, :, cp]) - torch.einsum('eoi,ei->eo', b, xd[:, :, cm])
+            om = torch.einsum('eoi,ei->eo', b, xd[:, :, cp]) + torch.einsum('eoi,ei->eo', a, xd[:, :, cm])
+            o = torch.stack([op, om], dim=1)
+        outs = o if outs is None else outs + o
+    return outs
+
+
+def zgemm_problem(mode, Co, E, seg_shapes, seed=0, x_scale=1.0, positive=False, device='cuda'):
+    """Random operands of one zgemm launch.  seg_shapes: [(Ci, ncomp, cplus, cminus, Kp)].  Returns (segs in the form ops.zgemm
+    takes, weight image, per-edge scales sx, float64 reference [E, planes, Co])."""
+    import torch
+    from se3_transformer_pytorch_b200 import ops
+    g = torch.Generator(device=device).manual_seed(seed)
+    rnd = (lambda *s: torch.rand(*s, generator=g, device=device) + 0.1) if positive else (lambda *s: torch.randn(*s, generator=g, device=device))
+    segs_ref, segs_k, parts = [], [], []
+    for Ci, nc, cp, cm, Kp in seg_shapes:
+        U = torch.zeros(E, 64, device=device)
+        U[:, :Kp] = rnd(E, Kp)
+        U[:, Kp - 1] = 1.0                                             # the bias slot
+        Fp = rnd(Co * Ci * min(mode, 2), Kp) / (Ci * Kp) ** 0.5
+        xp = rnd(E, Ci, nc) * x_scale
+        segs_ref.append((U, Fp, xp, cp, cm))
+        X = x_tile_layout(xp)
+        for kc in range(Kp // 16):
+            segs_k.append((U[:, 16 * kc:], X, Ci, nc, cp, cm))
+        parts.append((Fp.contiguous(), Ci))
+    img, S = ops.zgemm_image(parts, Co, mode)
+    # per-edge power-of-two scales as the model makes them (from the row maximum), exercising the scale / unscale path
+    rowmax = torch.stack([s[2].abs().amax(dim=(1, 2)) for s in segs_ref]).amax(0)
+    sx = torch.exp2(torch.floor(9 - torch.log2(rowmax.clamp(min=1e-30)))).float()
+    return segs_k, img, sx, zgemm_reference(mode, segs_ref, Co)
+
+
+def run_zgemm(mode, Co, E, seg_shapes, flush=0, seed=0, x_scale=1.0, positive=False):
+    """One zgemm launch on zgemm_problem's operands.  Returns (gpu out [E, planes, Co], float64 reference)."""
+    import torch
+    from se3_transformer_pytorch_b200 import ops
+    segs, img, sx, ref = zgemm_problem(mode, Co, E, seg_shapes, seed, x_scale, positive)
+    planes = min(mode, 2)
+    out = torch.full((E, planes, Co), 7.0, device=sx.device)
+    ops.zgemm(segs, img, sx, E, Co, mode, out, planes * Co, [0, Co], flush_stages=flush)
+    torch.cuda.synchronize()
+    return out, ref
+
+
+def zgemm_split_units(segs, Co, mode, flush_stages=0):
+    """The split units of a zgemm launch (its largest k_split)."""
+    from se3_transformer_pytorch_b200 import ops
+    arr = (ops.ZSeg * len(segs))(*[ops.ZSeg(U.data_ptr(), X.data_ptr(), Ci, nc, cp, cm) for U, X, Ci, nc, cp, cm in segs])
+    return ops.lib().se3_zgemm_split_units(arr, len(segs), Co, mode, flush_stages)
+
+
+def attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale):
+    """float64 attention of one degree: q [b,n,H*Dh,M]; kd, vd [b,n,J,kvh*Dh,M] with the prefix keys (global, null, self)
+    first and the K neighbours last; nmask [b,n,K] or None -> [b,n,H*Dh,M]."""
+    b, n, J, _, M = kd.shape
+    qh = q.reshape(b, n, H, Dh, M).astype(np.float64)
+    kh = np.broadcast_to(kd.reshape(b, n, J, kvh, Dh, M), (b, n, J, H, Dh, M)) if kvh == 1 else kd.reshape(b, n, J, H, Dh, M)
+    vh = np.broadcast_to(vd.reshape(b, n, J, kvh, Dh, M), (b, n, J, H, Dh, M)) if kvh == 1 else vd.reshape(b, n, J, H, Dh, M)
+    sim = np.einsum('bihdm,bijhdm->bihj', qh, kh.astype(np.float64)) * scale
+    if nmask is not None:
+        mk = np.concatenate([np.ones((b, n, J - nmask.shape[-1]), dtype=bool), nmask], -1)[:, :, None]
+        sim = np.where(mk, sim, -np.finfo(np.float32).max)
+    sim = sim - sim.max(-1, keepdims=True)
+    a = np.exp(sim); a /= a.sum(-1, keepdims=True)
+    return np.einsum('bihj,bijhdm->bihdm', a, vh.astype(np.float64)).reshape(b, n, H * Dh, M)

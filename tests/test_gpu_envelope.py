@@ -6,11 +6,11 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import DEG_CASES, GOLDEN, load_case, rel_err
-from test_gpu_kernels import (_attention_reference, test_norm_se3 as _norm_case, test_pairwise_lowrank_matches_fp64 as _pairwise_lr_case,
+from helpers import DEG_CASES, GOLDEN, attention_reference, load_case, rel_err, run_zgemm
+from test_gpu_kernels import (test_norm_se3 as _norm_case, test_pairwise_lowrank_matches_fp64 as _pairwise_lr_case,
                               test_pairwise_simt as _pairwise_simt_case, test_pairwise_tc_matches_fp64 as _pairwise_tc_case)
 from test_gpu_model import build_model, check_outputs, run_model
-from test_gpu_zgemm import (DEV, _run_zgemm, test_linear_tc_matches_fp64 as _linear_tc_case, test_rotate_pool as _rotate_pool_case,
+from test_gpu_zgemm import (DEV, test_linear_tc_matches_fp64 as _linear_tc_case, test_rotate_pool as _rotate_pool_case,
                             test_rotgather as _rotgather_case)
 
 pytestmark = pytest.mark.gpu
@@ -86,7 +86,7 @@ def test_attention_templates_match_fp64(Dh, M, H, K, b, n, opts):
     nmask = _mask(rng, b, n, K, opts)
     kw, kd, vd = _keys(rng, b, n, M, Ckv, k, v, opts)
     scale = Dh ** -0.5
-    ref = _attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale)
+    ref = attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale)
     got = ops.attention(cu(q), cu(k), cu(v), heads=H, dim_head=Dh, scale=scale, kv_heads=kvh,
                         nmask=None if nmask is None else cu(nmask), **{key: cu(t) for key, t in kw.items()}).cpu().numpy()
     err = _row_err(got, ref, H)
@@ -96,7 +96,7 @@ def test_attention_templates_match_fp64(Dh, M, H, K, b, n, opts):
 # ------------------------------------------------------------------ se3_attn_aligned_fwd: every degree and register width, long lists
 def _aligned_case(M, Dh, H, K, b, n, k_aligned, opts, seed):
     """Keys / values in the edge frames (component major, as zgemm writes them) against float64: rotate to the global frame in
-    float64, then attend as _attention_reference does."""
+    float64, then attend as attention_reference does."""
     from se3_transformer_pytorch_b200 import ops
     rng = np.random.default_rng(seed)
     kvh = 1 if opts.get('one_headed') else H
@@ -111,7 +111,7 @@ def _aligned_case(M, Dh, H, K, b, n, k_aligned, opts, seed):
     nmask = _mask(rng, b, n, K, opts)
     kw, kd, vd = _keys(rng, b, n, M, Ckv, kg, vg, opts)
     scale = Dh ** -0.5
-    ref = _attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale)
+    ref = attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale)
     got = ops.attention(cu(q), cu(kp if k_aligned else kg.astype(np.float32)), cu(vp), heads=H, dim_head=Dh, scale=scale,
                         kv_heads=kvh, nmask=None if nmask is None else cu(nmask), D=cu(Dm), k_aligned=k_aligned,
                         **{key: cu(t) for key, t in kw.items()}).cpu().numpy()
@@ -190,7 +190,7 @@ def test_zgemm_high_degree_segments(mode, Co, E, segs):
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, Co, 1):
         pytest.skip('needs sm_90')
-    out, ref = _run_zgemm(mode, Co, E, segs, seed=Co + mode)
+    out, ref = run_zgemm(mode, Co, E, segs, seed=Co + mode)
     err = rel_err(out.cpu().numpy(), ref.cpu().numpy())
     assert err < (6e-6 if mode == 3 else 3e-6), f'{err:.3e}'
 

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import GOLDEN, load_case, rel_err, decode_T, assert_graph_equal
+from helpers import GOLDEN, load_case, rel_err, decode_T, assert_graph_equal, attention_reference
 from oracle import se3_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -336,22 +336,6 @@ def test_pairwise_tc_headline_width_matches_simt():
 
 
 # ------------------------------------------------------------------ K5
-def _attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale):
-    """float64 attention of one degree: q [b,n,H*Dh,M]; kd, vd [b,n,J,kvh*Dh,M] with the prefix keys (global, null, self)
-    first and the K neighbours last; nmask [b,n,K] or None -> [b,n,H*Dh,M]."""
-    b, n, J, _, M = kd.shape
-    qh = q.reshape(b, n, H, Dh, M).astype(np.float64)
-    kh = np.broadcast_to(kd.reshape(b, n, J, kvh, Dh, M), (b, n, J, H, Dh, M)) if kvh == 1 else kd.reshape(b, n, J, H, Dh, M)
-    vh = np.broadcast_to(vd.reshape(b, n, J, kvh, Dh, M), (b, n, J, H, Dh, M)) if kvh == 1 else vd.reshape(b, n, J, H, Dh, M)
-    sim = np.einsum('bihdm,bijhdm->bihj', qh, kh.astype(np.float64)) * scale
-    if nmask is not None:
-        mk = np.concatenate([np.ones((b, n, J - nmask.shape[-1]), dtype=bool), nmask], -1)[:, :, None]
-        sim = np.where(mk, sim, -np.finfo(np.float32).max)
-    sim = sim - sim.max(-1, keepdims=True)
-    a = np.exp(sim); a /= a.sum(-1, keepdims=True)
-    return np.einsum('bihj,bijhdm->bihdm', a, vh.astype(np.float64)).reshape(b, n, H * Dh, M)
-
-
 @pytest.mark.parametrize('M,Dh,H,K,opts', [
     (1, 8, 2, 5, dict(self_kv=True)), (3, 24, 8, 8, dict(self_kv=True, mask=True)), (7, 64, 8, 16, dict(self_kv=True, mask=True)),
     (5, 16, 4, 33, dict()), (1, 8, 2, 4, dict(self_kv=True, null=True, G=3, mask=True)), (3, 8, 4, 6, dict(one_headed=True, self_kv=True, null=True)),
@@ -390,7 +374,7 @@ def test_attention(M, Dh, H, K, opts):
         vd = np.concatenate([np.broadcast_to(gv[:, None], (b, n, opts['G'], Ckv, M)), vd], 2)
         kw.update(global_k=cu(gk), global_v=cu(gv))
     scale = Dh ** -0.5
-    ref = _attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale)
+    ref = attention_reference(q, kd, vd, nmask, H, Dh, kvh, scale)
     got = ops.attention(cu(q), cu(k_nodes) if opts.get('lin_keys') else cu(k), cu(v), heads=H, dim_head=Dh, scale=scale,
                         nmask=None if nmask is None else cu(nmask), k_idx=cu(idx) if opts.get('lin_keys') else None,
                         kv_heads=kvh, **kw).cpu().numpy()

@@ -5,68 +5,10 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import rel_err
+from helpers import rel_err, run_zgemm
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-
-
-def _x_layout(xp):
-    """x' [E, Ci, ncomp] -> kernel layout [tiles][Ci][ncomp][128] (zero rows past E)."""
-    E, Ci, nc = xp.shape
-    tiles = (E + 127) // 128
-    buf = torch.zeros(tiles * 128, Ci, nc, dtype=torch.float32, device=xp.device)
-    buf[:E] = xp
-    return buf.reshape(tiles, 128, Ci, nc).permute(0, 2, 3, 1).contiguous().reshape(-1)
-
-
-def _zgemm_reference(mode, segs, Co):
-    """float64: segs = [(U [E,Kp], Fp [Co*Ci*F, Kp], x' [E,Ci,ncomp], cplus, cminus)] -> out [E, mode, Co]."""
-    outs = None
-    mode = min(mode, 2)                                              # mode 3 computes what mode 2 computes (Gauss form)
-    for U, Fp, xp, cp, cm in segs:
-        E, Ci = xp.shape[0], xp.shape[1]
-        Fv = Fp.double().reshape(Co, Ci, mode, -1)
-        Ud = U.double()[:, :Fv.shape[-1]]
-        w = torch.einsum('ek,oifk->eoif', Ud, Fv)                     # the radial weights of this segment
-        xd = xp.double()
-        if mode == 1:
-            o = torch.einsum('eoi,ei->eo', w[..., 0], xd[:, :, cp])[:, None]
-        else:
-            a, b = w[..., 0], w[..., 1]
-            op = torch.einsum('eoi,ei->eo', a, xd[:, :, cp]) - torch.einsum('eoi,ei->eo', b, xd[:, :, cm])
-            om = torch.einsum('eoi,ei->eo', b, xd[:, :, cp]) + torch.einsum('eoi,ei->eo', a, xd[:, :, cm])
-            o = torch.stack([op, om], dim=1)
-        outs = o if outs is None else outs + o
-    return outs
-
-
-def _run_zgemm(mode, Co, E, seg_shapes, flush=0, seed=0, x_scale=1.0, positive=False):
-    """seg_shapes: [(Ci, ncomp, cplus, cminus, Kp)].  Returns (gpu out [E, mode, Co], float64 reference)."""
-    from se3_transformer_pytorch_b200 import ops
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    rnd = (lambda *s: torch.rand(*s, generator=g, device=DEV) + 0.1) if positive else (lambda *s: torch.randn(*s, generator=g, device=DEV))
-    segs_ref, segs_k, parts = [], [], []
-    for Ci, nc, cp, cm, Kp in seg_shapes:
-        U = torch.zeros(E, 64, device=DEV)
-        U[:, :Kp] = rnd(E, Kp)
-        U[:, Kp - 1] = 1.0                                             # the bias slot
-        Fp = rnd(Co * Ci * min(mode, 2), Kp) / (Ci * Kp) ** 0.5
-        xp = rnd(E, Ci, nc) * x_scale
-        segs_ref.append((U, Fp, xp, cp, cm))
-        X = _x_layout(xp)
-        for kc in range(Kp // 16):
-            segs_k.append((U[:, 16 * kc:], X, Ci, nc, cp, cm))
-        parts.append((Fp.contiguous(), Ci))
-    img, S = ops.zgemm_image(parts, Co, mode)
-    # per-edge power-of-two scales as the model makes them (from the row maximum), exercising the scale / unscale path
-    rowmax = torch.stack([s[2].abs().amax(dim=(1, 2)) for s in segs_ref]).amax(0)
-    sx = torch.exp2(torch.floor(9 - torch.log2(rowmax.clamp(min=1e-30)))).float()
-    planes = min(mode, 2)
-    out = torch.full((E, planes, Co), 7.0, device=DEV)
-    ops.zgemm(segs_k, img, sx, E, Co, mode, out, planes * Co, [0, Co], flush_stages=flush)
-    torch.cuda.synchronize()
-    return out, _zgemm_reference(mode, segs_ref, Co)
 
 
 @pytest.mark.parametrize('mode,Co,E,segs', [
@@ -86,7 +28,7 @@ def test_zgemm_matches_fp64(mode, Co, E, segs, flush):
     from se3_transformer_pytorch_b200 import ops
     if not ops.tc_supported(DEV, Co, 1):
         pytest.skip('needs sm_90')
-    out, ref = _run_zgemm(mode, Co, E, segs, flush=flush, seed=flush)
+    out, ref = run_zgemm(mode, Co, E, segs, flush=flush, seed=flush)
     err = rel_err(out.cpu().numpy(), ref.cpu().numpy())
     assert err < (6e-6 if mode == 3 else 3e-6), f'flush={flush}: {err:.3e}'
 
@@ -98,7 +40,7 @@ def test_zgemm_is_scale_invariant(x_scale):
     if not ops.tc_supported(DEV, 128, 1):
         pytest.skip('needs sm_90')
     for mode in (2, 3):
-        out, ref = _run_zgemm(mode, 128, 200, [(8, 3, 2, 0, 16)], x_scale=x_scale)
+        out, ref = run_zgemm(mode, 128, 200, [(8, 3, 2, 0, 16)], x_scale=x_scale)
         assert rel_err(out.cpu().numpy(), ref.cpu().numpy()) < 6e-6
 
 
@@ -111,9 +53,9 @@ def test_zgemm_headline_width_long_k(mode):
     if not ops.tc_supported(DEV, 512, 1):
         pytest.skip('needs sm_90')
     segs = [(512, 2 * l + 1, l + (1 if mode >= 2 and l else 0), l - (1 if mode >= 2 and l else 0), 16) for l in ((0, 1, 2, 3) if mode == 1 else (1, 2, 3))]
-    out, ref = _run_zgemm(mode, 512, 512, segs, flush=0, positive=True)
+    out, ref = run_zgemm(mode, 512, 512, segs, flush=0, positive=True)
     err = rel_err(out.cpu().numpy(), ref.cpu().numpy())
-    out2, _ = _run_zgemm(mode, 512, 512, segs, flush=1 << 20, positive=True)
+    out2, _ = run_zgemm(mode, 512, 512, segs, flush=1 << 20, positive=True)
     err_nodrain = rel_err(out2.cpu().numpy(), ref.cpu().numpy())
     print(f'zgemm mode {mode} long-K positive operands: rel err {err:.3e} (default drain), {err_nodrain:.3e} (never drained)')
     import json, os

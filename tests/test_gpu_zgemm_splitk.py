@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from gen_zgemm_hashes import FIXTURE, cases, digest, run_case
+from helpers import zgemm_split_units
 
 CASES = cases()
 with open(FIXTURE) as _f:
@@ -32,9 +33,7 @@ def _run(name, k_split):
 
 
 def _units(segs, w_img, sx, E, Co, mode, out, out_edge_stride, comp_off, flush_stages=0, **_):
-    from se3_transformer_pytorch_b200 import ops
-    arr = (ops.ZSeg * len(segs))(*[ops.ZSeg(U.data_ptr(), X.data_ptr(), Ci, nc, cp, cm) for U, X, Ci, nc, cp, cm in segs])
-    return ops.lib().se3_zgemm_split_units(arr, len(segs), Co, mode, flush_stages)
+    return zgemm_split_units(segs, Co, mode, flush_stages)
 
 
 def _need_sm90():
