@@ -118,6 +118,22 @@ int se3_knn_rows_paged_fwd(const float* pool, const int* pages, const uint8_t* n
                            int64_t* out_idx, int64_t* out_col, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist,
                            void* stream);
 
+/* A paged decoding step padded to `rows` rows (replayed from a CUDA graph) is described by one device buffer, desc, laid out for
+ * num_clouds clouds: int64 cu_rows [num_clouds + 1], n_prev, k_per_cloud, pair_off, table_off [num_clouds each], then the int32
+ * page ids.  The step's B <= num_clouds clouds come first; clouds past them are empty (cu_rows = M, the step's rows), and
+ * 1 <= M <= rows.  pair_off[c] is where cloud c's [m_c, n_cur_c] pair rows start in the step's concatenated pair inputs.
+ *
+ * se3_decode_plan_fwd writes out int64 [4, rows]: for each row t < M of cloud c, node pos = n_prev[c] + r of its cloud, its
+ * pool row pages[table_off[c] + pos / page_size] * page_size + pos % page_size, its pair row pair_off[c] + r * n_cur_c and c.
+ * A padding row t >= M takes row M - 1's position, pair row and cloud, and pool row scratch_row + t - M.
+ * se3_knn_rows_paged_bucket_fwd is se3_knn_rows_paged_fwd over `rows` CTAs reading desc; padding row t >= M repeats the
+ * search of row M - 1 into its own output row.  n_max (any bound on n_cur_c, such as the pool's node count) sizes shared
+ * memory.  Neither reads anything back, so both can be captured in a CUDA graph. */
+int se3_decode_plan_fwd(const int64_t* desc, int num_clouds, int rows, int page_size, int64_t scratch_row, int64_t* out, void* stream);
+int se3_knn_rows_paged_bucket_fwd(const float* pool, const int64_t* desc, const uint8_t* neighbor_mask, int num_clouds, int rows,
+                                  int page_size, int n_max, int K, float valid_radius, int causal, int64_t* out_idx, int64_t* out_col,
+                                  uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream);
+
 /* Position of every neighbour in a sparse pair list (as in se3_pairs; batch_stride 0 when shared, else n): out[b,i,kk] = p with
  * cols[p] == idx[b,i,kk] inside row (b, i), or -1 if the row lacks that column.  idx, out: [b, n, k] int64.  The caller indexes
  * the list's values (edge tokens, edge features, hop counts) with a zero row appended for -1. */

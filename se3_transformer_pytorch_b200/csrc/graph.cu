@@ -325,7 +325,10 @@ knn_rows_kernel(const float* __restrict__ coors, const uint8_t* __restrict__ nod
 // The ragged form of knn_rows_kernel for clouds kept in pages of P nodes of one pool, coors [pages, P, 3] (PagedCausalDecoder):
 // cloud c's page ids are pages[table_off[c] ..], and its node j is pool row pages[table_off[c] + j / P] P + j % P.  out_idx
 // gets that pool row, out_col the column j; everything else is as in knn_rows_kernel.  table_off < 2^31.
-template <int THREADS>
+// BUCKET (a decoding step replayed from a CUDA graph): the grid has a fixed number of CTAs, at least the step's rows M =
+// cu_rows[num_clouds], and clouds past the step's are empty (cu_rows = M).  CTA t >= M is a padding row: it repeats the search
+// of row M - 1 and writes its own output row t.
+template <int THREADS, bool BUCKET>
 __global__ void __launch_bounds__(THREADS, 6)
 knn_rows_paged_kernel(const float* __restrict__ pool, const int* __restrict__ pages, const uint8_t* __restrict__ nbr,
                       const int64_t* __restrict__ cu_rows, const int64_t* __restrict__ n_prev, const int64_t* __restrict__ k_per_cloud,
@@ -333,7 +336,8 @@ knn_rows_paged_kernel(const float* __restrict__ pool, const int* __restrict__ pa
                       unsigned magic, unsigned shift, int K, float valid_radius, int causal, int64_t* __restrict__ out_idx, int64_t* __restrict__ out_col,
                       uint8_t* __restrict__ out_mask, float* __restrict__ out_rel_pos, float* __restrict__ out_rel_dist) {
   extern __shared__ unsigned long long keys[];
-  const int64_t t = blockIdx.x;
+  int64_t t = blockIdx.x;
+  if constexpr (BUCKET) t = min(t, cu_rows[num_clouds] - 1);
   int lo = 0, hi = num_clouds - 1;                  // the last cloud with cu_rows[lo] <= t
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
@@ -343,7 +347,7 @@ knn_rows_paged_kernel(const float* __restrict__ pool, const int* __restrict__ pa
   const int i = (int)(n_prev[lo] + r);
   const int n_c = (int)(n_prev[lo] + cu_rows[lo + 1] - cu_rows[lo]);
   const uint8_t* row_mask = nbr && pair_off[lo] >= 0 ? nbr + pair_off[lo] + r * n_c : nullptr;
-  const int64_t o = t * K;
+  const int64_t o = (BUCKET ? (int64_t)blockIdx.x : t) * K;
   const PagedCoords c{pool, pages, (int)table_off[lo], P, magic, shift};
   knn_row<THREADS>(keys, c, n_c, i, (int)k_per_cloud[lo], knn_npad(n_c), DensePairs{row_mask, nullptr}, nullptr, valid_radius,
                    causal, K, 0, out_idx + o, out_mask + o, out_rel_pos + o * 3, out_rel_dist + o);
@@ -516,6 +520,58 @@ extern "C" int se3_knn_rows_packed_fwd(const float* coors, const uint8_t* neighb
                          rows, K, valid_radius, causal, out_idx, out_mask, out_rel_pos, out_rel_dist, stream);
 }
 
+namespace se3 {
+// knn_rows_paged_kernel over `rows` CTAs; n_max: the longest searched cloud, which sizes shared memory (K slots per row)
+template <bool BUCKET>
+static int launch_knn_rows_paged(const float* pool, const int* pages, const uint8_t* nbr, const int64_t* cu_rows,
+                                 const int64_t* n_prev, const int64_t* k_per_cloud, const int64_t* pair_off, const int64_t* table_off,
+                                 int num_clouds, int64_t rows, int page_size, int n_max, int K, float valid_radius, int causal,
+                                 int64_t* out_idx, int64_t* out_col, uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist,
+                                 void* stream) {
+  constexpr int THREADS = 256;
+  const int key_words = n_max - 1 > KNN_TILE ? KNN_TILE + next_pow2(K) : knn_npad(n_max);
+  const size_t smem = (size_t)key_words * sizeof(unsigned long long);
+  unsigned magic, shift;
+  page_divisor((unsigned)page_size, magic, shift);
+  auto kernel = knn_rows_paged_kernel<THREADS, BUCKET>;
+  if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<(unsigned)rows, THREADS, smem, as_stream(stream)>>>(pool, pages, nbr, cu_rows, n_prev, k_per_cloud, pair_off, table_off,
+                                                               num_clouds, (unsigned)page_size, magic, shift, K, valid_radius, causal,
+                                                               out_idx, out_col, out_mask, out_rel_pos, out_rel_dist);
+  SE3_LAUNCH_OK();
+  return SE3_OK;
+}
+
+// One thread per row t of a decoding step padded to `rows` rows (see se3_decode_plan_fwd).  The row's cloud is found as
+// knn_rows_paged_kernel finds it, and its pool row with the same PagedCoords::row, so the plan and the search agree on every
+// row; padding rows t >= M take row M - 1's position, cloud and pair row, and scratch pool row scratch_row + t - M.
+__global__ void decode_plan_kernel(const int64_t* __restrict__ desc, int num_clouds, int rows, unsigned P, unsigned magic,
+                                   unsigned shift, int64_t scratch_row, int64_t* __restrict__ out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= rows) return;
+  const int64_t* cu_rows = desc;
+  const int64_t* n_prev = desc + num_clouds + 1;
+  const int64_t* pair_off = desc + 3 * num_clouds + 1;
+  const int64_t* table_off = desc + 4 * num_clouds + 1;
+  const int* pages = reinterpret_cast<const int*>(desc + 5 * num_clouds + 1);
+  const int64_t M = cu_rows[num_clouds];
+  const int64_t s = min((int64_t)t, M - 1);
+  int lo = 0, hi = num_clouds - 1;                  // the last cloud with cu_rows[lo] <= s
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (cu_rows[mid] <= s) lo = mid; else hi = mid - 1;
+  }
+  const int64_t r = s - cu_rows[lo];
+  const int64_t n_cur = n_prev[lo] + cu_rows[lo + 1] - cu_rows[lo];
+  const int pos = (int)(n_prev[lo] + r);
+  const PagedCoords c{nullptr, pages, (int)table_off[lo], P, magic, shift};
+  out[t] = pos;
+  out[rows + t] = t < M ? c.row(pos) : scratch_row + (t - M);
+  out[2 * rows + t] = pair_off[lo] + r * n_cur;
+  out[3 * rows + t] = lo;
+}
+}  // namespace se3
+
 extern "C" int se3_knn_rows_paged_fwd(const float* pool, const int* pages, const uint8_t* neighbor_mask, const int64_t* cu_rows,
                                       const int64_t* n_prev, const int64_t* k_per_cloud, const int64_t* pair_off,
                                       const int64_t* table_off, int num_clouds, int64_t rows, int page_size, int n_max, int K,
@@ -530,19 +586,43 @@ extern "C" int se3_knn_rows_paged_fwd(const float* pool, const int* pages, const
   SE3_REQUIRE(page_size >= 1, "se3_knn_rows_paged_fwd: page_size must be >= 1 (got %d)", page_size);
   SE3_REQUIRE(n_max > 1, "se3_knn_rows_paged_fwd: need n_max > 1 (got %d)", n_max);
   SE3_REQUIRE(K >= 1 && K <= KNN_TILE, "se3_knn_rows_paged_fwd: K must be in [1, %d] (got %d)", KNN_TILE, K);
-  constexpr int THREADS = 256;
-  const int key_words = n_max - 1 > KNN_TILE ? KNN_TILE + next_pow2(K) : knn_npad(n_max);
-  const size_t smem = (size_t)key_words * sizeof(unsigned long long);
+  return launch_knn_rows_paged<false>(pool, pages, neighbor_mask, cu_rows, n_prev, k_per_cloud, pair_off, table_off, num_clouds, rows,
+                                      page_size, n_max, K, valid_radius, causal, out_idx, out_col, out_mask, out_rel_pos,
+                                      out_rel_dist, stream);
+}
+
+extern "C" int se3_decode_plan_fwd(const int64_t* desc, int num_clouds, int rows, int page_size, int64_t scratch_row, int64_t* out,
+                                   void* stream) {
+  using namespace se3;
+  SE3_REQUIRE(desc && out, "se3_decode_plan_fwd: null pointer");
+  SE3_REQUIRE(num_clouds > 0 && rows >= num_clouds, "se3_decode_plan_fwd: need 0 < num_clouds <= rows (got %d clouds, %d rows)",
+              num_clouds, rows);
+  SE3_REQUIRE(page_size >= 1 && scratch_row >= 0, "se3_decode_plan_fwd: need page_size >= 1 and scratch_row >= 0 (got %d, %lld)",
+              page_size, (long long)scratch_row);
   unsigned magic, shift;
   page_divisor((unsigned)page_size, magic, shift);
-  auto kernel = knn_rows_paged_kernel<THREADS>;
-  if (smem > 48 * 1024) SE3_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kernel<<<(unsigned)rows, THREADS, smem, as_stream(stream)>>>(pool, pages, neighbor_mask, cu_rows, n_prev, k_per_cloud, pair_off,
-                                                               table_off, num_clouds, (unsigned)page_size, magic, shift, K,
-                                                               valid_radius, causal, out_idx, out_col, out_mask, out_rel_pos,
-                                                               out_rel_dist);
+  const int threads = 128;
+  decode_plan_kernel<<<(unsigned)ceil_div(rows, threads), threads, 0, as_stream(stream)>>>(desc, num_clouds, rows, (unsigned)page_size,
+                                                                                           magic, shift, scratch_row, out);
   SE3_LAUNCH_OK();
   return SE3_OK;
+}
+
+extern "C" int se3_knn_rows_paged_bucket_fwd(const float* pool, const int64_t* desc, const uint8_t* neighbor_mask, int num_clouds,
+                                             int rows, int page_size, int n_max, int K, float valid_radius, int causal,
+                                             int64_t* out_idx, int64_t* out_col, uint8_t* out_mask, float* out_rel_pos,
+                                             float* out_rel_dist, void* stream) {
+  using namespace se3;
+  SE3_REQUIRE(pool && desc && out_idx && out_col && out_mask && out_rel_pos && out_rel_dist, "se3_knn_rows_paged_bucket_fwd: null pointer");
+  SE3_REQUIRE(num_clouds > 0 && rows >= num_clouds, "se3_knn_rows_paged_bucket_fwd: need 0 < num_clouds <= rows (got %d clouds, %d rows)",
+              num_clouds, rows);
+  SE3_REQUIRE(page_size >= 1, "se3_knn_rows_paged_bucket_fwd: page_size must be >= 1 (got %d)", page_size);
+  SE3_REQUIRE(n_max > 1, "se3_knn_rows_paged_bucket_fwd: need n_max > 1 (got %d)", n_max);
+  SE3_REQUIRE(K >= 1 && K <= KNN_TILE, "se3_knn_rows_paged_bucket_fwd: K must be in [1, %d] (got %d)", KNN_TILE, K);
+  const int B = num_clouds;
+  return launch_knn_rows_paged<true>(pool, reinterpret_cast<const int*>(desc + 5 * B + 1), neighbor_mask, desc, desc + B + 1,
+                                     desc + 2 * B + 1, desc + 3 * B + 1, desc + 4 * B + 1, B, rows, page_size, n_max, K, valid_radius,
+                                     causal, out_idx, out_col, out_mask, out_rel_pos, out_rel_dist, stream);
 }
 
 extern "C" int se3_pair_lookup_fwd(const int64_t* row_ptr, const int* cols, int64_t nnz, int64_t batch_stride, const int64_t* idx,

@@ -2344,10 +2344,14 @@ class PackedCausalDecoder(_DecoderStages):
         returns for those M rows: {'d': [M, C, 2d+1]} ('0': [M, C]), or one degree with return_type."""
         ids, seqlens = self._check(ids, seqlens, feats, coors, edges, neighbor_mask, return_pooled)
         self._reserve(ids, seqlens, coors)
-        out = self.model._checked(lambda: self._step(ids, seqlens, feats, coors, edges, neighbor_mask, return_type))
+        out = self._run(ids, seqlens, feats, coors, edges, neighbor_mask, return_type)
         for c, m in zip(ids, seqlens):
             self._len[c] += m
         return out
+
+    def _run(self, ids, seqlens, feats, coors, edges, neighbor_mask, return_type):
+        """The step's outputs, once its cache room is reserved: its body and the check of its low-rank plans."""
+        return self.model._checked(lambda: self._step(ids, seqlens, feats, coors, edges, neighbor_mask, return_type))
 
     def _reserve(self, ids, seqlens, coors):
         """Room in the cache for the step, made once before its body (which a low-rank plan miss runs again).  The rows of this
@@ -2535,10 +2539,65 @@ class PageTables:
             self.tables[c] += [self._take() for _ in range(f)]
         return copies
 
+    def rollback(self, plan, ids, copies):
+        """Undo commit(plan, ids), which returned copies, when it did not grow the pool: tables, counts and the free list are
+        as they were before it.  Pages go back to the free list in the reverse order of their taking."""
+        for c, f in reversed(list(zip(ids, plan.fresh))):
+            for _ in range(f):
+                p = self.tables[c].pop()
+                self.refs[p] = 0
+                self.free.append(p)
+        for (c, at, _), (old, new, _) in reversed(list(zip(plan.cow, copies))):
+            self.tables[c][at] = old
+            self.refs[old] += 1
+            self.refs[new] = 0
+            self.free.append(new)
+
     def _take(self):
         p = self.free.pop()
         self.refs[p] = 1
         return p
+
+
+DECODE_GRAPH_ROWS = 64        # most rows of a paged decoding step that is replayed from a CUDA graph
+
+
+def decode_graph_bucket(max_nodes, n_prev, seqlens, ks):
+    """The CUDA-graph bucket (M rounded up to a power of two, K) of a step of a PagedCausalDecoder built with max_nodes that
+    appends seqlens[c] nodes to clouds of n_prev[c] nodes with k_c = ks[c] neighbours, or None if the step runs eagerly: a
+    decoder without max_nodes (its pool moves when it grows), a cloud in its first call (a prompt), more than DECODE_GRAPH_ROWS
+    rows or clouds with different k_c."""
+    M = sum(seqlens)
+    if max_nodes is None or min(n_prev) == 0 or M > DECODE_GRAPH_ROWS or len(set(ks)) != 1:
+        return None
+    return 1 << (M - 1).bit_length(), ks[0]
+
+
+class _DecodeGraph:
+    """One captured step of a PagedCausalDecoder for a bucket of rows (M_bucket) and neighbours (K), and the static buffers it
+    reads: the descriptor (pinned on the host, and its device copy), the features, coordinates and pair inputs of M_bucket rows
+    (pair inputs concatenated per cloud, room for M_bucket rows of n_pos columns), and the outputs and deferred low-rank
+    checks it writes."""
+
+    def __init__(self, rows, K, n_pos, page_ids, feats, coors, edges, neighbor_mask):
+        dev = coors.device
+        self.rows, self.K, self.room = rows, K, page_ids
+        self.out_dtype = coors.dtype if coors.dtype == torch.float64 else None       # as SE3Transformer._compute_dtype
+        words = ops.decode_desc_words(rows, page_ids)
+        self.host_desc = torch.zeros(words, dtype=torch.int32).pin_memory()
+        self.desc = torch.zeros(words, dtype=torch.int32, device=dev)
+        static = lambda t: torch.zeros((rows,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
+        self.feats = {d: static(v) for d, v in feats.items()} if isinstance(feats, dict) else static(feats)
+        self.coors = torch.zeros((rows, 3), dtype=torch.float32, device=dev)
+        self.edges = self.nbr = None
+        if edges is not None:
+            e = edges[0]
+            dtype = e.dtype if not e.is_floating_point() else torch.float32
+            self.edges = torch.zeros((rows * n_pos,) + tuple(e.shape[2:]), dtype=dtype, device=dev)
+        if neighbor_mask is not None:
+            self.nbr = torch.zeros(rows * n_pos, dtype=torch.uint8, device=dev)
+        self.copied = torch.cuda.Event()          # recorded after each replay: its descriptor copy is done
+        self.graph = self.out = self.checks = None
 
 
 class PagedCausalDecoder(PackedCausalDecoder):
@@ -2566,6 +2625,14 @@ class PagedCausalDecoder(PackedCausalDecoder):
         self._book = PageTables(self.page_size, None if max_nodes is None else -(-self.max_nodes // self.page_size))
         self._next_id = 0
         self._len = {}                            # open cloud id -> number of nodes
+        # CUDA-graph steps (max_nodes only, DESIGN.md 10.3): padding rows store into scratch pages after the pool's
+        self._scratch_pages = 0 if max_nodes is None else -(-DECODE_GRAPH_ROWS // self.page_size)
+        self._graphs = {}                         # (M_bucket, K, input kind) -> _DecodeGraph
+        self._graph_pool = None                   # the memory pool the graphs share (they never run at the same time)
+        self._graph_sw = self._graph_plans = None     # the switches and low-rank plans the graphs were captured with
+        self._commit = None                       # the last step's page plan, ids and copies (PageTables.rollback)
+        self.graph_replays = 0                    # steps replayed from a graph
+        self.graph_capture_s = {}                 # (M_bucket, K) -> seconds its last capture took (with its warm-up step)
 
     def pages_in_use(self):
         """Distinct pages that open clouds reference."""
@@ -2613,6 +2680,7 @@ class PagedCausalDecoder(PackedCausalDecoder):
         ops._require_cuda(coors)
         self._grow(plan.reserved, coors.device)
         copies = self._book.commit(plan, ids)
+        self._commit = (plan, ids, copies)
         if copies:
             P = self.page_size
             rows = torch.tensor([[old * P + r for old, _, n in copies for r in range(n)],
@@ -2625,9 +2693,11 @@ class PagedCausalDecoder(PackedCausalDecoder):
         return [self.coors] + [t for feats, nodemax in self.stages.values() for t in (*feats.values(), nodemax)]
 
     def _grow(self, pages, dev):
-        """A pool of `pages` pages, the old pool copied to its first pages (page ids do not change)."""
-        if self.coors is not None and pages <= self.coors.shape[0]:
+        """A pool of `pages` pages, the old pool copied to its first pages (page ids do not change).  A fixed pool has scratch
+        pages after them, which no cloud owns: the padding rows of graph steps store there."""
+        if self.coors is not None and pages + self._scratch_pages <= self.coors.shape[0]:
             return
+        pages += self._scratch_pages
 
         def grown(t):
             new = t.new_empty((pages,) + tuple(t.shape[1:]))
@@ -2651,3 +2721,170 @@ class PagedCausalDecoder(PackedCausalDecoder):
                                                                 ks, self.model._valid_radius(), causal=True,
                                                                 neighbor_mask=neighbor_mask)
         return where, idx, col, nmask, rel_pos, rel_dist
+
+    # ---- steps replayed from CUDA graphs (DESIGN.md 10.3) -----------------------------------------------------------------
+    def drop_graphs(self):
+        """Forget every captured step and the memory they share; the next eligible step of each bucket captures again."""
+        self._graphs.clear()
+        self._graph_pool = self._graph_sw = self._graph_plans = None
+
+    def _plan_state(self, sw):
+        """What the captured steps read of every ConvSE3's decisions: its weight pack, low-rank plan and whether it left it.
+        Holding it keeps the plan's tensors, which the graphs read, alive."""
+        state = []
+        for conv in self.model.conv_modules():
+            pk = conv.packed(sw)
+            state.append((pk, pk['lr'], conv._lr_blocked))
+        return state
+
+    @staticmethod
+    def _same_plans(a, b):
+        return all(x[0] is y[0] and x[1] is y[1] and x[2] == y[2] for x, y in zip(a, b))
+
+    def _desc_room(self, need, rows):
+        """Page ids a bucket's descriptor has room for: the step's need rounded up to a power of two (at least 1024), at most
+        rows * max_pages (each listed cloud reads at most max_pages).  A later step that needs more captures the bucket again."""
+        return min(max(1024, 1 << (need - 1).bit_length()), rows * self._book.max_pages)
+
+    def _graph_key(self, ids, seqlens, feats, coors, edges, neighbor_mask, return_type, sw):
+        """(M_bucket, K, the kind of inputs) of a step to replay from a graph, or None if it runs eagerly."""
+        if sw.no_decode_graphs or not self.stages:
+            return None
+        n_prev = [self._len[c] for c in ids]
+        bucket = decode_graph_bucket(self.max_nodes, n_prev, seqlens, [self.model._num_neighbors(p + m, 0) for p, m in zip(n_prev, seqlens)])
+        if bucket is None:
+            return None
+        rows, K = bucket
+        if ops.lowrank_enabled(rows * K, sw) != ops.lowrank_enabled(sum(seqlens) * K, sw):
+            return None                           # the capture decides the route for rows * K edges, the step has fewer
+        kind = (tuple((d, tuple(v.shape[1:]), v.dtype) for d, v in sorted(feats.items())) if isinstance(feats, dict) else
+                (tuple(feats.shape[1:]), feats.dtype))
+        pairs = None if edges is None else (tuple(edges[0].shape[2:]), edges[0].is_floating_point())
+        return rows, K, kind, coors.dtype, pairs, neighbor_mask is not None, return_type
+
+    def _run(self, ids, seqlens, feats, coors, edges, neighbor_mask, return_type):
+        sw = switches.current()
+        key = self._graph_key(ids, seqlens, feats, coors, edges, neighbor_mask, return_type, sw)
+        if key is None:
+            return super()._run(ids, seqlens, feats, coors, edges, neighbor_mask, return_type)
+        if self._graphs and (sw != self._graph_sw or not self._same_plans(self._plan_state(sw), self._graph_plans)):
+            self.drop_graphs()                    # a switch or a low-rank plan changed since the capture
+        P = self.page_size
+        need = sum(-(-(self._len[c] + m) // P) for c, m in zip(ids, seqlens))
+        g = self._graphs.get(key)
+        if g is not None and need > g.room:       # the descriptor outgrew its room: capture the bucket again with more
+            del self._graphs[key]
+            if not self._graphs:
+                self.drop_graphs()
+            g = None
+        fresh = g is None
+        if fresh:
+            g = _DecodeGraph(key[0], key[1], self._n_pos(), self._desc_room(need, key[0]), feats, coors, edges, neighbor_mask)
+        elif not g.copied.query():
+            g.copied.synchronize()                # the previous replay still reads the pinned descriptor (no checks waited)
+        M = self._fill(g, ids, seqlens, feats, coors, edges, neighbor_mask)
+        if fresh:
+            self._capture(g, key, return_type, sw)
+        g.graph.replay()
+        g.copied.record()
+        self.graph_replays += 1
+        bad = check_lowrank_stats(g.checks)       # the one host synchronisation of a replayed step
+        if bad:
+            self.drop_graphs()
+            if any(conv.free_master for conv in bad):
+                self._book.rollback(*self._commit)
+                raise LowRankPlanMiss('low-rank radial plan does not cover this input; pack_weights(max_distance=...) was given too '
+                                      'small a distance')
+            return super()._run(ids, seqlens, feats, coors, edges, neighbor_mask, return_type)
+        if isinstance(g.out, dict):
+            return {d: v[:M].clone() for d, v in g.out.items()}
+        return g.out[:M].clone()
+
+    def _n_pos(self):
+        """A bound on every cloud's length: the nodes of the pool's pages."""
+        return self._book.max_pages * self.page_size
+
+    def _fill(self, g, ids, seqlens, feats, coors, edges, neighbor_mask):
+        """The step's descriptor and inputs into g's static buffers (no host synchronisation); returns its rows M."""
+        P = self.page_size
+        n_prev = [self._len[c] for c in ids]
+        n_cur = [p + m for p, m in zip(n_prev, seqlens)]
+        tables = [self._book.tables[c][:-(-n // P)] for c, n in zip(ids, n_cur)]
+        M = ops.fill_decode_desc(g.host_desc, g.rows, n_prev, seqlens, [g.K] * len(ids), tables)
+        if isinstance(feats, dict):
+            for d, v in feats.items():
+                g.feats[d][:M].copy_(v, non_blocking=True)
+        else:
+            g.feats[:M].copy_(feats, non_blocking=True)
+        g.coors[:M].copy_(coors, non_blocking=True)
+        for buf, per_cloud in ((g.edges, edges), (g.nbr, neighbor_mask)):
+            if per_cloud is not None:
+                flat = torch.cat([t.reshape((-1,) + tuple(t.shape[2:])) for t in per_cloud])
+                buf[:flat.shape[0]].copy_(flat, non_blocking=True)
+        return M
+
+    def _capture(self, g, key, return_type, sw):
+        """Warm up g's step outside the capture (weight images, plans and library state are built there), then capture it."""
+        import time
+        t0 = time.perf_counter()
+        dev = g.coors.device
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):
+            self._graph_body(g, return_type)
+        torch.cuda.current_stream(dev).wait_stream(side)
+        plans = self._plan_state(sw)
+        if self._graphs and not self._same_plans(plans, self._graph_plans):
+            self.drop_graphs()                    # the warm-up rebuilt a low-rank plan that the other graphs read
+        if self._graph_pool is None:
+            self._graph_pool = torch.cuda.graph_pool_handle()
+        g.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g.graph, pool=self._graph_pool):
+            g.out, g.checks = self._graph_body(g, return_type)
+        self._graphs[key] = g
+        self._graph_sw, self._graph_plans = sw, plans
+        self.graph_capture_s[key[:2]] = time.perf_counter() - t0
+
+    def _graph_body(self, g, return_type):
+        """_step over g's static buffers, every per-row tensor built on the device from the descriptor: (outputs, deferred
+        checks).  Rows M .. M_bucket pad the step: they repeat row M - 1's search and store into the scratch pages."""
+        model, rows, K, n_pos = self.model, g.rows, g.K, self._n_pos()
+        out_dtype = g.out_dtype
+        if model.output_degrees == 1:
+            return_type = 0
+        g.desc.copy_(g.host_desc, non_blocking=True)
+        desc = g.desc.view(torch.int64)
+        pos, where, pair_row, _ = ops.decode_plan(desc, rows, rows, self.page_size, n_pos)
+        if isinstance(g.feats, dict):
+            feats = {d: v.unsqueeze(0) for d, v in g.feats.items()}
+        else:
+            feats = model._embed_tokens(g.feats.unsqueeze(0), pos)
+            feats = {'0': feats[..., None]}
+        feats = model._check_features(feats, g.coors)
+        self.coors.view(-1, 3).index_copy_(0, where, g.coors)
+        idx, col, nmask, rel_pos, rel_dist = ops.knn_rows_paged_bucket(self.coors, desc, rows, rows, n_pos, K, model._valid_radius(),
+                                                                       causal=True, neighbor_mask=g.nbr)
+        e = model._edge_features(None if g.edges is None else g.edges[pair_row[:, None] + col], None)
+        pos_emb = None
+        if exists(model.rotary_pos_emb):
+            pos_emb = model._rotary(pos.view(1, rows), torch.cat((pos[:, None], col), dim=1).view(1, rows, 1 + K), n_pos,
+                                    rel_dist.view(1, rows, K))
+        geom = Geometry(rel_pos[None], model.num_degrees - 1, deferred=[])
+        step = dict(dest=where, rows=_StepRows(rows), edge_info=(idx[None], nmask[None], None if e is None else e[None]),
+                    rel_dist=rel_dist[None], geom=geom)
+        out, checks = self._walk(feats, step, pos_emb, lambda v: v[0], out_dtype, return_type)
+        # An eager step rebuilds a plan that its ConvSE3 can still rebuild (masters kept) once the step's largest distance
+        # exceeds the plan's range D (ConvSE3.lowrank_plan).  The replay keeps the captured plan, so such a step counts as a
+        # plan miss: the graphs are dropped and the step runs eagerly.  Padding rows repeat row M - 1, so the maximum over the
+        # bucket is the step's; it is compared in float64, as lowrank_plan compares float(rel_dist.max()) with D.
+        d_max, seen = None, set()
+        for conv, _, _ in list(checks):
+            if conv.free_master or id(conv) in seen:
+                continue
+            seen.add(id(conv))
+            if d_max is None:
+                d_max = rel_dist.max().double()
+            beyond = torch.where(d_max > conv._packed['lr']['D'], 1e30, 0.0).float()
+            checks.append((conv, torch.stack((beyond, torch.ones_like(beyond))).view(1, 2),
+                           torch.ones(1, dtype=torch.bool, device=beyond.device)))
+        return out, checks

@@ -27,6 +27,8 @@ _SIGNATURES = {
     'se3_knn_rows_fwd': (c_int, [c_void_p] * 3 + [c_int, c_int64, c_int64, c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 5),
     'se3_knn_rows_packed_fwd': (c_int, [c_void_p] * 7 + [c_int, c_int64, c_int64, c_int, c_int, c_float, c_int] + [c_void_p] * 5),
     'se3_knn_rows_paged_fwd': (c_int, [c_void_p] * 8 + [c_int, c_int64, c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 6),
+    'se3_decode_plan_fwd': (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p]),
+    'se3_knn_rows_paged_bucket_fwd': (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_float, c_int] + [c_void_p] * 6),
     'se3_pair_lookup_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
@@ -433,6 +435,72 @@ def knn_rows_paged(pool, tables, n_prev, seqlens, k, valid_radius, *, neighbor_m
         _check(lib().se3_knn_rows_paged_fwd(_p(pool), _p(page_ids), _p(nbr), _p(cu_d), _p(prev_d), _p(k_d), _p(off_d), _p(toff_d),
                                             B, M, P, max(n_cur), K, float(min(valid_radius, 3.0e38)), int(bool(causal)), _p(idx),
                                             _p(col), _p(mask), _p(rel_pos), _p(rel_dist), _stream()))
+    return idx, col, mask.view(torch.bool), rel_pos, rel_dist
+
+
+def decode_desc_words(num_clouds, page_ids):
+    """int32 words of the descriptor of a padded paged decoding step (se3b200.h, se3_decode_plan_fwd) for num_clouds clouds
+    and room for page_ids page ids, rounded up to whole int64 words."""
+    return 2 * (5 * num_clouds + 1) + page_ids + page_ids % 2
+
+
+def fill_decode_desc(buf, num_clouds, n_prev, seqlens, k, tables):
+    """Write the descriptor of a step that appends seqlens[c] nodes to cloud c of n_prev[c] nodes with k[c] neighbours into the
+    int32 host tensor buf (decode_desc_words long): cu_rows, n_prev, k, pair_off and table_off for num_clouds clouds, those past
+    the step's empty, then the page ids of tables[c] (the ones the step reads, in node order).  Returns the step's rows M."""
+    B, nd = len(seqlens), 5 * num_clouds + 1
+    if not 1 <= B <= num_clouds or not len(n_prev) == len(k) == len(tables) == B:
+        raise ValueError(f'fill_decode_desc: need 1 <= {B} clouds <= num_clouds = {num_clouds}, one n_prev, k and table each')
+    words = buf.numpy()
+    head = words[:2 * nd].view(np.int64)
+    m = np.asarray(seqlens, dtype=np.int64)
+    n_cur = np.asarray(n_prev, dtype=np.int64) + m
+    lens = np.fromiter((len(t) for t in tables), dtype=np.int64, count=B)
+    if 2 * nd + int(lens.sum()) > words.shape[0]:
+        raise ValueError(f'fill_decode_desc: {int(lens.sum())} page ids exceed the descriptor\'s room of {words.shape[0] - 2 * nd}')
+    head[:] = 0
+    head[1:B + 1] = np.cumsum(m)
+    head[B + 1:num_clouds + 1] = head[B]
+    head[num_clouds + 1:num_clouds + 1 + B] = n_prev
+    head[2 * num_clouds + 1:3 * num_clouds + 1] = 1
+    head[2 * num_clouds + 1:2 * num_clouds + 1 + B] = k
+    head[3 * num_clouds + 2:3 * num_clouds + 1 + B] = np.cumsum(m * n_cur)[:-1]
+    head[4 * num_clouds + 2:4 * num_clouds + 1 + B] = np.cumsum(lens)[:-1]
+    words[2 * nd:2 * nd + int(lens.sum())] = [p for t in tables for p in t]
+    return int(head[B])
+
+
+def decode_plan(desc, num_clouds, rows, page_size, scratch_row):
+    """Per row of a paged decoding step padded to `rows` rows, from its device descriptor (fill_decode_desc): int64 [4, rows] of
+    the node's position in its cloud, its pool row, where its pair row starts in the step's concatenated pair inputs, and its
+    cloud.  Padding rows repeat the last row, except for their pool rows scratch_row, scratch_row + 1, ..."""
+    _require_cuda(desc)
+    out = torch.empty((4, rows), dtype=torch.int64, device=desc.device)
+    with torch.cuda.device(desc.device), _timed('decode_plan', nbytes=64 * rows):
+        _check(lib().se3_decode_plan_fwd(_p(desc), num_clouds, rows, page_size, scratch_row, _p(out), _stream()))
+    return out
+
+
+def knn_rows_paged_bucket(pool, desc, num_clouds, rows, n_max, K, valid_radius, *, neighbor_mask=None, causal=False):
+    """knn_rows_paged of a step padded to `rows` rows, described by its device descriptor (fill_decode_desc) instead of host
+    lists: every cloud has k = K; neighbor_mask: None or the step's masks concatenated as bytes at the descriptor's pair_off.
+    n_max bounds every cloud's length.  Padding rows repeat the last row's search.  Nothing is read back."""
+    _require_cuda(pool, desc, neighbor_mask)
+    if pool.dtype != torch.float32 or not pool.is_contiguous() or pool.dim() != 3 or pool.shape[2] != 3:
+        raise ValueError('knn_rows_paged_bucket: pool must be a contiguous float32 [pages, page_size, 3] tensor')
+    if K > KNN_MAX_K:
+        raise ValueError(f'knn_rows_paged_bucket: {K} neighbours exceed {KNN_MAX_K}, the longest list the tiled search keeps')
+    dev = pool.device
+    idx = torch.empty((rows, K), dtype=torch.int64, device=dev)
+    col = torch.empty((rows, K), dtype=torch.int64, device=dev)
+    mask = torch.empty((rows, K), dtype=torch.uint8, device=dev)
+    rel_pos = torch.empty((rows, K, 3), dtype=torch.float32, device=dev)
+    rel_dist = torch.empty((rows, K), dtype=torch.float32, device=dev)
+    nbr = _u8(neighbor_mask)
+    with torch.cuda.device(dev), _timed('knn_rows_paged', nbytes=33 * rows * K):
+        _check(lib().se3_knn_rows_paged_bucket_fwd(_p(pool), _p(desc), _p(nbr), num_clouds, rows, pool.shape[1], n_max, K,
+                                                   float(min(valid_radius, 3.0e38)), int(bool(causal)), _p(idx), _p(col), _p(mask),
+                                                   _p(rel_pos), _p(rel_dist), _stream()))
     return idx, col, mask.view(torch.bool), rel_pos, rel_dist
 
 

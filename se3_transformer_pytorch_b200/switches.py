@@ -24,6 +24,8 @@ implementations of the same forward (or tunes one); none changes what the model 
 |                             |                   |                  | attention block may take: its edge work runs over node chunks     |
 |                             |                   |                  | sized to fit (model.plan_node_chunks; the result is bit-identical)|
 |                             |                   |                  | unset: a quarter of the device's total memory; 0: one-node chunks |
+| SE3B200_NO_DECODE_GRAPHS    | no_decode_graphs  | off              | every step of a paged decoder with max_nodes runs eagerly, none   |
+|                             |                   |                  | is replayed from a CUDA graph (DESIGN.md 10.3; same rows)         |
 
 The model reads `current()` once per ConvSE3 dispatch, LinearSE3 / AttentionSE3 call, Geometry and pack_weights; ConvSE3
 rebuilds its cached dispatch decisions when a switch they depend on changes.  A captured CUDA graph (GraphedForward) replays
@@ -53,6 +55,7 @@ class Switches:
     z_flush: int = None
     z_flush_mult: int = 1
     edge_budget_mb: float = None
+    no_decode_graphs: bool = False
 
     def zgemm_flush(self, mode):
         """flush_stages of se3_zgemm_fwd: 0 (the library's default) unless SE3B200_Z_FLUSH or SE3B200_Z_FLUSH_MULT is set."""
