@@ -134,6 +134,17 @@ int se3_knn_rows_paged_bucket_fwd(const float* pool, const int64_t* desc, const 
                                   int page_size, int n_max, int K, float valid_radius, int causal, int64_t* out_idx, int64_t* out_col,
                                   uint8_t* out_mask, float* out_rel_pos, float* out_rel_dist, void* stream);
 
+/* Node digests of a prefix-cache lookup (PagedCausalDecoder with prefix_cache, DESIGN.md 10.4).  Rows are concatenated per cloud
+ * as in se3_knn_rows_packed_fwd (cu_rows [num_clouds + 1], n_prev [num_clouds]); row t of cloud c is node
+ * i = n_prev[c] + t - cu_rows[c].  feats [rows, width] is each row's conv_in input (every input degree, flattened and
+ * concatenated), coors [rows, 3].  The pair inputs, if any, are concatenated per cloud as [m_c, n_cur_c] entries starting at
+ * entry pair_off[c]: edge_tokens int64, or edge_values float32 with edge_dim values per entry (at most one of the two), and
+ * neighbor_mask one byte per entry; only columns j < i are read.  out [rows, 2] gets each node's two 64-bit digest lanes, a
+ * function of the exact bits of those inputs only (the formula is in DESIGN.md 10.4), whatever the launch geometry. */
+int se3_prefix_keys_fwd(const float* feats, int64_t rows, int64_t width, const float* coors, const int64_t* edge_tokens,
+                        const float* edge_values, int edge_dim, const uint8_t* neighbor_mask, const int64_t* cu_rows,
+                        const int64_t* n_prev, const int64_t* pair_off, int num_clouds, uint64_t* out, void* stream);
+
 /* Position of every neighbour in a sparse pair list (as in se3_pairs; batch_stride 0 when shared, else n): out[b,i,kk] = p with
  * cols[p] == idx[b,i,kk] inside row (b, i), or -1 if the row lacks that column.  idx, out: [b, n, k] int64.  The caller indexes
  * the list's values (edge tokens, edge features, hop counts) with a zero row appended for -1. */

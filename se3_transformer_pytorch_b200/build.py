@@ -16,7 +16,7 @@ TAG = os.environ.get('SE3B200_LIB_TAG', '')
 EXTRA_DEFS = os.environ.get('SE3B200_NVCC_DEFS', '').split()
 LIB = os.path.join(PKG, f'libse3b200{TAG}.so')
 STAMP = os.path.join(PKG, f'.libse3b200{TAG}.stamp')
-SOURCES = ['api.cu', 'graph.cu', 'basis.cu', 'radial.cu', 'tbuild.cu', 'pairwise_simt.cu', 'pairwise_tc.cu', 'pairwise_lr.cu', 'zgemm.cu', 'aligned.cu', 'attention.cu', 'elementwise.cu']
+SOURCES = ['api.cu', 'graph.cu', 'basis.cu', 'radial.cu', 'tbuild.cu', 'pairwise_simt.cu', 'pairwise_tc.cu', 'pairwise_lr.cu', 'zgemm.cu', 'aligned.cu', 'attention.cu', 'elementwise.cu', 'prefix.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '--use_fast_math=false',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-O2']
 

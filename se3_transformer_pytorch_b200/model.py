@@ -9,10 +9,12 @@ libse3b200.so through `ops`; the cheap glue around it (embeddings, LinearSE3 GEM
 Forward only: everything runs under torch.no_grad().  CUDA only: there is no CPU fallback.
 """
 import numbers
+import collections
 import operator
 from math import sqrt
 from typing import NamedTuple
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -1394,17 +1396,22 @@ class SE3Transformer(nn.Module):
         doing the edge work of its new nodes only."""
         return CausalDecoder(self, batch_size)
 
-    def packed_decoder(self, page_size=None, max_nodes=None):
+    def packed_decoder(self, page_size=None, max_nodes=None, prefix_cache=False):
         """An empty PackedCausalDecoder of this causal model: clouds of different lengths decoded together, each opened, extended,
         truncated, forked and closed on its own, every step carrying the new nodes of any subset of them.  With an integer
         page_size >= 1, a PagedCausalDecoder instead, the same decoder with its cache in pages of page_size nodes: memory follows
         the nodes decoded and forks share their prefix; max_nodes (pages for that many nodes, reserved at the first step) caps
-        its pool, which otherwise doubles when full."""
+        its pool, which otherwise doubles when full.  prefix_cache=True (paged only) shares the full pages of equal prompts
+        between clouds opened separately (DESIGN.md 10.4)."""
+        if not isinstance(prefix_cache, bool):
+            raise ValueError(f'packed_decoder: prefix_cache must be a bool, got {prefix_cache!r}')
         if page_size is None:
             if max_nodes is not None:
                 raise ValueError('packed_decoder: max_nodes caps the pages of a paged cache; give a page_size too')
+            if prefix_cache:
+                raise ValueError('packed_decoder: the prefix cache shares pages of a paged cache; give a page_size too')
             return PackedCausalDecoder(self)
-        return PagedCausalDecoder(self, page_size, max_nodes)
+        return PagedCausalDecoder(self, page_size, max_nodes, prefix_cache)
 
     # ---- forward ----------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -2063,7 +2070,11 @@ class _DecoderStages:
             x = ff(self._attend(i, attn_block, x, step, pos_emb))
         if exists(model.conv_out):
             x = self._conv(model.conv_out, 'out', x, step)
-        return model._output(x, reduce, out_dtype, return_type), step['geom'].deferred
+        return self._output(x, reduce, out_dtype, return_type, step), step['geom'].deferred
+
+    def _output(self, x, reduce, out_dtype, return_type, step):
+        """The step's outputs from the trunk's last features (SE3Transformer._output)."""
+        return self.model._output(x, reduce, out_dtype, return_type)
 
 
 class CausalDecoder(_DecoderStages):
@@ -2447,27 +2458,50 @@ class DecoderCacheFull(RuntimeError):
 
 class StepPages(NamedTuple):
     """What a step needs from PageTables.plan: the pool size after it, the copy-on-write pages (cloud, index in its table, rows
-    to copy) and the fresh pages each listed cloud appends."""
+    to copy), the fresh pages each listed cloud appends and, with a prefix cache, the cached pages each cloud in its first call
+    attaches ((cloud, pages), ...)."""
     reserved: int
     cow: list
     fresh: list
+    hits: tuple = ()
 
 
 class PageTables:
     """The page bookkeeping of a PagedCausalDecoder, on the host (it holds no tensors): each cloud's block table, the ids of the
     pages that hold its nodes [0, P), [P, 2P), ...; one reference count per page; and a free list.  The pool has `reserved`
     pages on the device; a page that no table references is free, and allocations take freed pages first (the most recent
-    first).  A cloud of n nodes has at least ceil(n / P) pages: more only after a step failed once its pages were taken."""
+    first).  A cloud of n nodes has at least ceil(n / P) pages: more only after a step failed once its pages were taken.
 
-    def __init__(self, page_size, max_pages=None):
+    With cache=True it also keeps the prefix cache (DESIGN.md 10.4): page key -> page, least recently used first.  The cache holds
+    one reference on each page it registers; a page only the cache holds is evictable (n_evictable counts them).  An allocation
+    takes a free page, else evicts the least recently used evictable page; only then does the pool grow (or a capped pool refuse
+    the step).  A page that a copy on write of the same commit copies from is never evicted by it.  A hit counts as a use once
+    its step succeeds (use).  rollback restores tables, counts and entries, except the entries the commit evicted: their pages may
+    already hold the failed step's rows, so they stay out of the cache and their pages are free."""
+
+    def __init__(self, page_size, max_pages=None, cache=False):
         self.P, self.max_pages = page_size, max_pages
         self.reserved = 0
-        self.refs = []                            # page id -> number of tables that hold it
+        self.refs = []                            # page id -> number of tables (and the cache) that hold it
         self.free = []                            # unreferenced page ids, taken from the end
         self.tables = {}                          # cloud -> page ids
+        self.cached = collections.OrderedDict() if cache else None      # page key -> page id, least recently used first
+        self.page_key = {}                        # cached page id -> its key
+        self.n_evictable = 0                      # cached pages that only the cache holds
+        self._victims = None                      # during a commit: its candidates for eviction, least recently used first
 
     def pages_in_use(self):
-        return self.reserved - len(self.free)
+        return self.reserved - len(self.free) - self.n_evictable
+
+    def pages_cached(self):
+        return 0 if self.cached is None else len(self.cached)
+
+    def _ref(self, p, delta):
+        """Add delta to page p's count, keeping n_evictable in step."""
+        r = self.refs[p]
+        self.refs[p] = r + delta
+        if p in self.page_key:
+            self.n_evictable += (r + delta == 1) - (r == 1)
 
     def open(self, cloud):
         self.tables[cloud] = []
@@ -2486,25 +2520,77 @@ class PageTables:
         """new shares the pages of cloud's first n nodes."""
         table = self.tables[cloud][:-(-n // self.P)]
         for p in table:
-            self.refs[p] += 1
+            self._ref(p, 1)
         self.tables[new] = list(table)
 
     def _drop(self, pages):
         for p in pages:
-            self.refs[p] -= 1
+            self._ref(p, -1)
             if not self.refs[p]:
                 self.free.append(p)
 
-    def plan(self, ids, n_prev, seqlens):
+    # ---- the prefix cache ------------------------------------------------------------------------------------------
+    def lookup(self, keys):
+        """The cached pages of keys[0], keys[1], ... up to the first miss (nothing changes)."""
+        pages = []
+        for key in keys:
+            p = self.cached.get(key) if self.cached else None
+            if p is None:
+                break
+            pages.append(p)
+        return pages
+
+    def use(self, pages):
+        """Mark the entries of these cached pages as the most recently used (a hit, once its step has succeeded)."""
+        for p in pages:
+            if p in self.page_key:
+                self.cached.move_to_end(self.page_key[p])
+
+    def register(self, key, page):
+        """Cache `page` (a full page of a prompt) under `key`, with one reference; a key already registered keeps its entry."""
+        if key in self.cached or page in self.page_key:
+            return
+        self.refs[page] += 1
+        self.cached[key] = page
+        self.page_key[page] = key
+        self.n_evictable += self.refs[page] == 1
+
+    def clear(self):
+        """Drop every entry and the cache's references."""
+        if self.cached:
+            pages = list(self.cached.values())
+            self.cached.clear()
+            self.page_key.clear()
+            self.n_evictable = 0
+            self._drop(pages)
+
+    def _evict(self, keep):
+        """Take the least recently used evictable page (none in keep) out of the cache; returns it, unreferenced and not on the
+        free list.  The candidates are listed once per commit: within a commit no page becomes evictable except the ones in keep."""
+        if self._victims is None:
+            self._victims = collections.deque(p for p in self.cached.values() if self.refs[p] == 1)
+        while True:
+            p = self._victims.popleft()
+            if p in self.page_key and self.refs[p] == 1 and p not in keep:
+                break
+        del self.cached[self.page_key.pop(p)]
+        self.n_evictable -= 1
+        self.refs[p] = 0
+        return p
+
+    # ---- steps -------------------------------------------------------------------------------------------------------
+    def plan(self, ids, n_prev, seqlens, hits=()):
         """The pages a step that appends seqlens[i] nodes to cloud ids[i] of n_prev[i] nodes needs (StepPages), without changing
         anything.  A step writes nodes >= n_prev only, so the one page of a cloud that it may write while another cloud holds it
         is the page of node n_prev, when n_prev is not a page boundary: that page is copied on write, its first n_prev % P rows.
         Clouds are planned in order, so of siblings that write one shared page in the same step the last writes it in place.
-        Raises DecoderCacheFull if a capped pool has too few free pages."""
+        hits: (cloud, cached pages) of clouds in their first call, which attach those pages (n_prev = len(pages) P).  Raises
+        DecoderCacheFull if a capped pool has too few free and evictable pages."""
         P = self.P
+        attach = dict(hits)
         refs, cow, fresh = {}, [], []
         for c, p, m in zip(ids, n_prev, seqlens):
-            table = self.tables[c]
+            table = attach.get(c, self.tables[c])
             if p % P:
                 page = table[p // P]
                 r = refs.get(page, self.refs[page])
@@ -2513,35 +2599,51 @@ class PageTables:
                     refs[page] = r - 1
             fresh.append(max(0, -(-(p + m) // P) - len(table)))
         need = len(cow) + sum(fresh)
+        hit_pages = {p for _, pages in hits for p in pages}
+        spare = len(self.free) + self.n_evictable - sum(self.refs[p] == 1 for p in hit_pages)
+        hits = tuple((c, tuple(pages)) for c, pages in hits)
         if self.max_pages is not None:
-            if need > len(self.free) + self.max_pages - self.reserved:
+            if need > spare + self.max_pages - self.reserved:
                 raise DecoderCacheFull(f'extend: the step needs {need} free pages of {P} nodes and the pool has '
-                                       f'{len(self.free) + self.max_pages - self.reserved} of {self.max_pages} (max_nodes); close, '
+                                       f'{spare + self.max_pages - self.reserved} of {self.max_pages} (max_nodes); close, '
                                        'truncate or pre-empt clouds and retry')
-            return StepPages(self.max_pages, cow, fresh)
-        short = need - len(self.free)
-        return StepPages(self.reserved if short <= 0 else max(2 * self.reserved, self.reserved + short), cow, fresh)
+            return StepPages(self.max_pages, cow, fresh, hits)
+        short = need - spare
+        return StepPages(self.reserved if short <= 0 else max(2 * self.reserved, self.reserved + short), cow, fresh, hits)
 
     def commit(self, plan, ids):
-        """Take the planned pages: grow the pool to plan.reserved, give each copy-on-write cloud a fresh page in place of the
-        shared one and append fresh pages.  Returns the copies [(old page, new page, rows)] that the caller makes on the device."""
+        """Take the planned pages: attach the cached pages of plan.hits, grow the pool to plan.reserved, give each copy-on-write
+        cloud a fresh page in place of the shared one and append fresh pages.  Returns the copies [(old page, new page, rows)]
+        that the caller makes on the device."""
+        self._victims = None
+        keep = set()                              # pages copied from: they must keep their rows until the copies are made
+        for c, pages in plan.hits:
+            self.tables[c] = list(pages)
+            for p in pages:
+                self._ref(p, 1)
         if plan.reserved > self.reserved:
-            self.free[:0] = range(plan.reserved - 1, self.reserved - 1, -1)      # new pages after the freed ones, lowest first
+            # every evictable page goes before the pool grows: the new pages come after the free and the evicted ones
+            evicted = [self._evict(keep) for _ in range(self.n_evictable)]
+            self.free[:0] = list(range(plan.reserved - 1, self.reserved - 1, -1)) + evicted[::-1]
             self.refs += [0] * (plan.reserved - self.reserved)
             self.reserved = plan.reserved
         copies = []
         for c, at, rows in plan.cow:
-            old, new = self.tables[c][at], self._take()
+            old = self.tables[c][at]
+            keep.add(old)
+            new = self._take(keep)
             self.tables[c][at] = new
-            self.refs[old] -= 1                   # still held by the cloud it was shared with
+            self._ref(old, -1)                    # still held by the cloud it was shared with (or the cache)
             copies.append((old, new, rows))
         for c, f in zip(ids, plan.fresh):
-            self.tables[c] += [self._take() for _ in range(f)]
+            self.tables[c] += [self._take(keep) for _ in range(f)]
+        self._victims = None
         return copies
 
     def rollback(self, plan, ids, copies):
-        """Undo commit(plan, ids), which returned copies, when it did not grow the pool: tables, counts and the free list are
-        as they were before it.  Pages go back to the free list in the reverse order of their taking."""
+        """Undo commit(plan, ids), which returned copies, when it did not grow the pool: tables, counts and the free list are as
+        they were before it, and so are the cache's entries except those it evicted, which stay evicted with their pages free
+        (the failed step may have written them).  Pages go back to the free list in the reverse order of their taking."""
         for c, f in reversed(list(zip(ids, plan.fresh))):
             for _ in range(f):
                 p = self.tables[c].pop()
@@ -2549,14 +2651,51 @@ class PageTables:
                 self.free.append(p)
         for (c, at, _), (old, new, _) in reversed(list(zip(plan.cow, copies))):
             self.tables[c][at] = old
-            self.refs[old] += 1
+            self._ref(old, 1)
             self.refs[new] = 0
             self.free.append(new)
+        for c, pages in reversed(plan.hits):
+            for p in pages:
+                self._ref(p, -1)
+            self.tables[c] = []
 
-    def _take(self):
-        p = self.free.pop()
+    def _take(self, keep=()):
+        p = self.free.pop() if self.free else self._evict(keep)
         self.refs[p] = 1
         return p
+
+
+PREFIX_SEEDS = (0x243F6A8885A308D3, 0x13198A2E03707344)         # se3_prefix_keys_fwd's lane seeds
+PREFIX_GOLD = 0x9E3779B97F4A7C15
+_U64 = (1 << 64) - 1
+
+
+def _mix64(z):
+    """splitmix64's finalizer on uint64 numpy arrays (wrapping)."""
+    z = z ^ (z >> np.uint64(30))
+    z = z * np.uint64(0xBF58476D1CE4E5B9)
+    z = z ^ (z >> np.uint64(27))
+    z = z * np.uint64(0x94D049BB133111EB)
+    return z ^ (z >> np.uint64(31))
+
+
+def prefix_page_keys(digests, P):
+    """The prefix-cache keys of the full pages of a prompt from its node digests (uint64 [n, 2], se3_prefix_keys_fwd): per
+    lane l, page q's digest is mix64(sum over its rows r of mix64(d[qP + r, l] + (r + 1) G)) and its key
+    key_q = mix64(key_{q-1} ^ digest_q) from key_{-1} = the lane seed, so a key names every node of the prefix up to its page.
+    Returns [(q, key lane 0, key lane 1)] for q < n // P, as Python ints."""
+    d = np.asarray(digests, dtype=np.uint64)
+    pages = d.shape[0] // P
+    if not pages:
+        return []
+    with np.errstate(over='ignore'):
+        r = (np.arange(1, P + 1, dtype=np.uint64) * np.uint64(PREFIX_GOLD))[None, :, None]
+        page = _mix64(_mix64(d[:pages * P].reshape(pages, P, 2) + r).sum(axis=1, dtype=np.uint64))
+        keys, k = [], np.array(PREFIX_SEEDS, dtype=np.uint64)
+        for q in range(pages):
+            k = _mix64(k ^ page[q])
+            keys.append((q, int(k[0]), int(k[1])))
+    return keys
 
 
 DECODE_GRAPH_ROWS = 64        # most rows of a paged decoding step that is replayed from a CUDA graph
@@ -2614,15 +2753,24 @@ class PagedCausalDecoder(PackedCausalDecoder):
     (PageTables.plan).  The pool doubles when it runs out of pages, or, with max_nodes, is fixed at ceil(max_nodes / P) pages
     and a step that does not fit raises DecoderCacheFull before any device work, leaving the decoder unchanged."""
 
-    def __init__(self, model, page_size, max_nodes=None):
+    def __init__(self, model, page_size, max_nodes=None, prefix_cache=False):
         _DecoderStages.__init__(self, model, 'packed_decoder')
         if isinstance(page_size, bool) or not isinstance(page_size, numbers.Integral) or page_size < 1:
             raise ValueError(f'packed_decoder: page_size must be None or an integer >= 1, got {page_size!r}')
         if max_nodes is not None and (isinstance(max_nodes, bool) or not isinstance(max_nodes, numbers.Integral) or max_nodes < 1):
             raise ValueError(f'packed_decoder: max_nodes must be None or an integer >= 1, got {max_nodes!r}')
+        if not isinstance(prefix_cache, bool):
+            raise ValueError(f'packed_decoder: prefix_cache must be a bool, got {prefix_cache!r}')
         self.page_size = int(page_size)
         self.max_nodes = None if max_nodes is None else int(max_nodes)
-        self._book = PageTables(self.page_size, None if max_nodes is None else -(-self.max_nodes // self.page_size))
+        self.prefix_cache = prefix_cache
+        self._book = PageTables(self.page_size, None if max_nodes is None else -(-self.max_nodes // self.page_size), prefix_cache)
+        # the prefix cache (DESIGN.md 10.4): every eager step's outputs per pool row, the state its entries were computed under,
+        # and how many nodes of each cloud came from it
+        self._out = None                          # {d: [pages, P, ...]} float32, before the dtype cast and return_type
+        self._out_rows = None                     # the rows of the running step that _out keeps (its prompts of a page or more)
+        self._cache_sw = self._cache_plans = None
+        self._prefix = {}
         self._next_id = 0
         self._len = {}                            # open cloud id -> number of nodes
         # CUDA-graph steps (max_nodes only, DESIGN.md 10.3): padding rows store into scratch pages after the pool's
@@ -2642,6 +2790,19 @@ class PagedCausalDecoder(PackedCausalDecoder):
         """Pages allocated on the device."""
         return self._book.reserved
 
+    def pages_cached(self):
+        """Pages the prefix cache holds, whether or not a cloud also references them."""
+        return self._book.pages_cached()
+
+    def clear_prefix_cache(self):
+        """Drop every prefix-cache entry; pages that no cloud references become free."""
+        self._book.clear()
+
+    def prefix_nodes(self, cloud):
+        """How many of the cloud's nodes came from the prefix cache (its first nodes)."""
+        self._known(cloud, 'prefix_nodes')
+        return min(self._prefix.get(cloud, 0), self._len[cloud])
+
     # ---- lifecycle -----------------------------------------------------------------------------------------
     def open(self, count=1):
         """count new empty clouds; returns their ids, increasing integers that are never reused."""
@@ -2658,12 +2819,15 @@ class PagedCausalDecoder(PackedCausalDecoder):
         """Forget a cloud; the pages only it held are free for the next allocation."""
         self._known(cloud, 'close')
         del self._len[cloud]
+        self._prefix.pop(cloud, None)
         self._book.close(cloud)
 
     def truncate(self, cloud, n):
         """Rewind a cloud to its first n nodes (0 <= n <= length) and drop its pages past them."""
         super().truncate(cloud, n)
         self._book.truncate(cloud, self._len[cloud])
+        if cloud in self._prefix:
+            self._prefix[cloud] = min(self._prefix[cloud], self._len[cloud])
 
     def fork(self, cloud):
         """A new cloud whose nodes so far are `cloud`'s, sharing its pages (no device work, nothing allocated); returns its id."""
@@ -2671,12 +2835,194 @@ class PagedCausalDecoder(PackedCausalDecoder):
         new = self.open()[0]
         self._len[new] = self._len[cloud]
         self._book.fork(cloud, new, self._len[cloud])
+        if cloud in self._prefix:
+            self._prefix[new] = self._prefix[cloud]
         return new
 
+    # ---- the prefix cache (DESIGN.md 10.4) -----------------------------------------------------------------------------
+    @torch.no_grad()
+    def extend(self, ids, seqlens, feats, coors, edges=None, neighbor_mask=None, return_type=None, return_pooled=False):
+        if not self.prefix_cache:
+            return super().extend(ids, seqlens, feats, coors, edges, neighbor_mask, return_type, return_pooled)
+        ids, seqlens = self._check(ids, seqlens, feats, coors, edges, neighbor_mask, return_pooled)
+        prompts = [i for i, c in enumerate(ids) if self._len[c] == 0]
+        self._commit = None
+        if not prompts:                           # a decode step: no lookup, nothing to register
+            out = self._attempt(lambda: (self._reserve(ids, seqlens, coors),
+                                         self._run(ids, seqlens, feats, coors, edges, neighbor_mask, return_type))[1], {})
+            for c, m in zip(ids, seqlens):
+                self._len[c] += m
+            return out
+        ops._require_cuda(coors)                  # the lookup runs on the device
+        sw = switches.current()
+        if self._book.cached and not self._cache_current(sw):
+            self._book.clear()                    # its rows were computed under other switches or plans
+        starts = [0]
+        for m in seqlens:
+            starts.append(starts[-1] + m)
+        keys, hits = self._lookup(ids, seqlens, starts, prompts, feats, coors, edges, neighbor_mask)
+        P = self.page_size
+        H = {c: len(pages) * P for c, pages in hits.items()}
+        sub = [(i, c) for i, c in enumerate(ids) if seqlens[i] > H.get(c, 0)]
+        sub_ids, sub_lens = [c for _, c in sub], [seqlens[i] - H.get(c, 0) for i, c in sub]
+        args = (feats, coors, edges, neighbor_mask)
+        if hits:                                  # the rest of the step: rows from n_prev = hP of each hit prompt
+            keep = torch.tensor([r for i, c in sub for r in range(starts[i] + H.get(c, 0), starts[i + 1])], dtype=torch.int64)
+            rows = lambda t: t[keep.to(t.device)]
+            per_cloud = lambda ts: None if ts is None else [ts[i][H.get(c, 0):] for i, c in sub]
+            args = ({d: rows(v) for d, v in feats.items()} if isinstance(feats, dict) else rows(feats), rows(coors),
+                    per_cloud(edges), per_cloud(neighbor_mask))
+        for c, h in H.items():
+            self._len[c] = h
+        kept, at = [], 0                          # the step rows of the prompts whose full pages may be registered
+        for (i, _), m in zip(sub, sub_lens):
+            if i in keys:
+                kept += range(at, at + m)
+            at += m
+        self._out_rows = torch.tensor(kept, dtype=torch.int64).to(coors.device) if kept else None
+        try:
+            out = self._attempt(lambda: (self._reserve(sub_ids, sub_lens, coors, tuple(hits.items())),
+                                         PackedCausalDecoder._run(self, sub_ids, sub_lens, *args, return_type) if sub_ids else None)[1],
+                                H)
+        finally:
+            self._out_rows = None
+        for c, m in zip(sub_ids, sub_lens):
+            self._len[c] += m
+        for i in prompts:
+            self._prefix[ids[i]] = H.get(ids[i], 0)
+        for pages in hits.values():
+            self._book.use(pages)
+        self._register(sw, ids, keys, hits)
+        if not hits:
+            return out
+        return self._assemble(ids, seqlens, starts, hits, sub, out, coors, return_type)
+
+    def _attempt(self, step, hits):
+        """Run step(); if it raises, undo its page commit (the cache's entries too) and the lengths of the hit clouds."""
+        try:
+            return step()
+        except BaseException:
+            if self._commit is not None:
+                self._rollback()
+            for c in hits:
+                self._len[c] = 0
+            raise
+
+    def _rollback(self):
+        self._book.rollback(*self._commit)
+        self._commit = None
+
+    def _cache_current(self, sw):
+        return sw == self._cache_sw and self._same_plans(self._plan_state(sw), self._cache_plans)
+
+    def _lookup(self, ids, seqlens, starts, prompts, feats, coors, edges, neighbor_mask):
+        """The page keys of every prompt of at least one page ({step index: [key of page 0, 1, ...]}), and the verified cached
+        pages each prompt attaches ({cloud: pages}): its keys looked up from page 0 to the first miss, then its stored coordinates
+        and conv_in rows compared bit for bit with the prompt's (one device comparison), stopping at the first page that differs."""
+        model, P, dev = self.model, self.page_size, coors.device
+        long = [i for i in prompts if seqlens[i] >= P]
+        if not long:
+            return {}, {}
+        lens = [seqlens[i] for i in long]
+        rows = torch.cat([torch.arange(starts[i], starts[i + 1]) for i in long])
+        # the conv_in input of the prompt rows, as _step builds it (positions count from 0 in a first call)
+        if isinstance(feats, dict):
+            x = {d: v[rows.to(v.device)].unsqueeze(0) for d, v in feats.items()}
+        else:
+            pos = torch.cat([torch.arange(m) for m in lens]).to(dev)
+            x = {'0': model._embed_tokens(feats[rows.to(feats.device)].unsqueeze(0), pos)[..., None]}
+        x = {d: v[0] for d, v in model._check_features(x, coors).items()}
+        R = rows.shape[0]
+        width = torch.cat([x[d].reshape(R, -1) for d in sorted(x, key=int)], dim=1)
+        xyz = coors[rows.to(dev)].float().contiguous()
+        pair = lambda ts, f: None if ts is None else [f(ts[i].to(dev)) for i in long]
+        e = pair(edges, lambda t: t.float() if t.is_floating_point() else t.long())
+        digests = ops.prefix_keys(width, xyz, lens, edges=e, neighbor_mask=pair(neighbor_mask, lambda t: t))
+        digests = digests.cpu().numpy().view(np.uint64)                # the one read-back of the keys
+        first = torch.tensor([0] + lens[:-1]).cumsum(0).tolist()          # each prompt's first row among the R
+        keys = {i: prefix_page_keys(digests[f:f + m], P) for i, f, m in zip(long, first, lens)}
+        cand = {i: (f, self._book.lookup(keys[i])) for i, f in zip(long, first)}
+        cand = {i: c for i, c in cand.items() if c[1]}
+        if not cand:
+            return keys, {}
+        pages = torch.tensor([p for _, pg in cand.values() for p in pg]).to(dev)
+        at = torch.tensor([f + r for f, pg in cand.values() for r in range(len(pg) * P)]).to(dev)
+        n = pages.shape[0]
+        same = lambda stored, new: (stored.reshape(n, -1).view(torch.int32) == new.reshape(n, -1).view(torch.int32)).all(1)
+        ok = same(self.coors[pages], xyz[at])
+        for d, t in self.stages['in'][0].items():
+            ok &= same(t[pages], x[d][at])
+        ok = ok.cpu().tolist()
+        hits, j = {}, 0
+        for i, (_, pg) in cand.items():
+            good = ok[j:j + len(pg)]
+            j += len(pg)
+            h = good.index(False) if False in good else len(good)
+            if h:
+                hits[ids[i]] = pg[:h]
+        return keys, hits
+
+    def _register(self, sw, ids, keys, hits):
+        """After a step that carried prompts: each prompt's full pages that the step wrote go into the cache under their keys,
+        tagged with the switches and plans they were computed under (entries of other ones are dropped first)."""
+        if not keys:
+            return
+        state = self._plan_state(sw)
+        if self._book.cached and not (sw == self._cache_sw and self._same_plans(state, self._cache_plans)):
+            self._book.clear()
+        self._cache_sw, self._cache_plans = sw, state
+        for i, page_keys in keys.items():
+            table = self._book.tables[ids[i]]
+            for q in range(len(hits.get(ids[i], ())), len(page_keys)):
+                self._book.register(page_keys[q], table[q])
+
+    def _assemble(self, ids, seqlens, starts, hits, sub, out, coors, return_type):
+        """The step's rows in ids order: the hit prompts' first hP rows from the cached outputs, the others from the step."""
+        P, dev = self.page_size, coors.device
+        out_dtype = self.model._compute_dtype(coors)
+        rt = 0 if self.model.output_degrees == 1 else return_type
+        where = {c: i for i, c in enumerate(ids)}
+        hit_at = torch.tensor([starts[where[c]] + r for c, pg in hits.items() for r in range(len(pg) * P)]).to(dev)
+        pool = torch.tensor([p * P + r for pg in hits.values() for p in pg for r in range(P)]).to(dev)
+        H = {c: len(pg) * P for c, pg in hits.items()}
+        sub_at = torch.tensor([r for i, c in sub for r in range(starts[i] + H.get(c, 0), starts[i + 1])], dtype=torch.int64).to(dev)
+        M = starts[-1]
+
+        def place(d, part):
+            v = self._out[d]
+            cached = v.view((-1,) + tuple(v.shape[2:]))[pool]
+            if exists(out_dtype):
+                cached = cached.to(out_dtype)
+            res = cached.new_empty((M,) + tuple(cached.shape[1:]))
+            res.index_copy_(0, hit_at, cached)
+            if part is not None:
+                res.index_copy_(0, sub_at, part)
+            return res
+        if exists(rt):
+            return place(str(rt), out)
+        return {d: place(d, None if out is None else out[d]) for d in self._out}
+
+    def _output(self, x, reduce, out_dtype, return_type, step):
+        """With the prefix cache, a step that carries prompts of a page or more (always eager) also keeps their rows of every
+        degree, in float32 before the dtype cast and return_type, at their pool rows: a later hit on their pages returns them."""
+        rows = self._out_rows
+        if rows is None:
+            return super()._output(x, reduce, out_dtype, return_type, step)
+        x = self.model._output(x, reduce, None, None)
+        if self._out is None:
+            self._out = {d: v.new_empty((self.coors.shape[0], self.page_size) + tuple(v.shape[1:])) for d, v in x.items()}
+        dest = step['dest'][rows]
+        for d, v in x.items():
+            self._out[d].view((-1,) + tuple(v.shape[1:])).index_copy_(0, dest, v[rows])
+        if exists(out_dtype):
+            x = {k: v.to(out_dtype) for k, v in x.items()}
+        return x[str(return_type)] if exists(return_type) else x
+
     # ---- one step ------------------------------------------------------------------------------------------
-    def _reserve(self, ids, seqlens, coors):
-        """Every page of the step, and its copies on write, before its body: the body must stay idempotent."""
-        plan = self._book.plan(ids, [self._len[c] for c in ids], seqlens)
+    def _reserve(self, ids, seqlens, coors, hits=()):
+        """Every page of the step, and its copies on write, before its body: the body must stay idempotent.  hits: the cached
+        pages that clouds in their first call attach (prefix cache)."""
+        plan = self._book.plan(ids, [self._len[c] for c in ids], seqlens, hits)
         ops._require_cuda(coors)
         self._grow(plan.reserved, coors.device)
         copies = self._book.commit(plan, ids)
@@ -2690,7 +3036,8 @@ class PagedCausalDecoder(PackedCausalDecoder):
                 flat.index_copy_(0, rows[1], flat.index_select(0, rows[0]))
 
     def _tensors(self):
-        return [self.coors] + [t for feats, nodemax in self.stages.values() for t in (*feats.values(), nodemax)]
+        return [self.coors] + [t for feats, nodemax in self.stages.values() for t in (*feats.values(), nodemax)] + \
+            list((self._out or {}).values())
 
     def _grow(self, pages, dev):
         """A pool of `pages` pages, the old pool copied to its first pages (page ids do not change).  A fixed pool has scratch
@@ -2707,6 +3054,8 @@ class PagedCausalDecoder(PackedCausalDecoder):
             self.coors = torch.empty((0, self.page_size, 3), dtype=torch.float32, device=dev)
         self.coors = grown(self.coors)
         self.stages = {name: ({d: grown(t) for d, t in feats.items()}, grown(nodemax)) for name, (feats, nodemax) in self.stages.items()}
+        if self._out is not None:
+            self._out = {d: grown(t) for d, t in self._out.items()}
 
     def _where(self, ids, lens, pos):
         """Each new row's pool row, table_c[pos // P] P + pos % P."""
@@ -2792,7 +3141,7 @@ class PagedCausalDecoder(PackedCausalDecoder):
         if bad:
             self.drop_graphs()
             if any(conv.free_master for conv in bad):
-                self._book.rollback(*self._commit)
+                self._rollback()
                 raise LowRankPlanMiss('low-rank radial plan does not cover this input; pack_weights(max_distance=...) was given too '
                                       'small a distance')
             return super()._run(ids, seqlens, feats, coors, edges, neighbor_mask, return_type)

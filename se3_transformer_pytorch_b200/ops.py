@@ -29,6 +29,7 @@ _SIGNATURES = {
     'se3_knn_rows_paged_fwd': (c_int, [c_void_p] * 8 + [c_int, c_int64, c_int, c_int, c_int, c_float, c_int] + [c_void_p] * 6),
     'se3_decode_plan_fwd': (c_int, [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p]),
     'se3_knn_rows_paged_bucket_fwd': (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_float, c_int] + [c_void_p] * 6),
+    'se3_prefix_keys_fwd': (c_int, [c_void_p, c_int64, c_int64] + [c_void_p] * 3 + [c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p]),
     'se3_pair_lookup_fwd': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_gather_pairs_fwd': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     'se3_basis_fwd': (c_int, [c_void_p, c_int64, c_int] + [c_void_p] * 5 + [c_int, c_void_p, c_void_p]),
@@ -502,6 +503,66 @@ def knn_rows_paged_bucket(pool, desc, num_clouds, rows, n_max, K, valid_radius, 
                                                    float(min(valid_radius, 3.0e38)), int(bool(causal)), _p(idx), _p(col), _p(mask),
                                                    _p(rel_pos), _p(rel_dist), _stream()))
     return idx, col, mask.view(torch.bool), rel_pos, rel_dist
+
+
+def prefix_keys(feats, coors, seqlens, n_prev=None, *, edges=None, neighbor_mask=None):
+    """Node digests of the prefix cache (se3_prefix_keys_fwd, DESIGN.md 10.4) of rows concatenated per cloud: feats [M, W]
+    float32, each row's conv_in input with its degrees flattened and concatenated; coors [M, 3] float32; seqlens and n_prev (default
+    zeros) per cloud; edges None or one [m_c, n_cur_c] int64 token or [m_c, n_cur_c, edge_dim] float32 tensor per cloud;
+    neighbor_mask None or one bool [m_c, n_cur_c] per cloud.  Node i of a cloud covers columns j < i of its pair rows only.
+    Returns int64 [M, 2]: the bits of each node's two uint64 lanes.  The descriptors go up in one copy; nothing is read back."""
+    if feats.dtype != torch.float32 or feats.dim() != 2 or coors.dtype != torch.float32 or tuple(coors.shape) != (feats.shape[0], 3):
+        raise ValueError('prefix_keys: feats must be float32 [M, W] and coors float32 [M, 3]')
+    masks = list(neighbor_mask) if neighbor_mask is not None else None
+    pairs = list(edges) if edges is not None else None
+    _require_cuda(feats, coors, *(masks or ()), *(pairs or ()))
+    seqlens = [int(m) for m in seqlens]
+    n_prev = [0] * len(seqlens) if n_prev is None else [int(p) for p in n_prev]
+    M, B = feats.shape[0], len(seqlens)
+    if B == 0 or len(n_prev) != B or min(seqlens) < 1 or min(n_prev) < 0 or sum(seqlens) != M:
+        raise ValueError(f'prefix_keys: need one seqlen >= 1 and n_prev >= 0 per cloud, summing to the {M} rows')
+    if M >= 2 ** 31:
+        raise ValueError(f'prefix_keys: {M} rows exceed the 1-D grid')
+    n_cur = [p + m for p, m in zip(n_prev, seqlens)]
+    off, at = [], 0                               # the pair rows of every cloud, [m_c, n_cur_c] entries each, end to end
+    for m, n in zip(seqlens, n_cur):
+        off.append(at)
+        at += m * n
+    nbr = None
+    if masks is not None:
+        if len(masks) != B or any(t is None or tuple(t.shape) != (m, n) for t, m, n in zip(masks, seqlens, n_cur)):
+            raise ValueError(f'prefix_keys: neighbor_mask must be a list of {B} per-cloud [m, n_cur] masks')
+        nbr = torch.cat([_u8(t).reshape(-1) for t in masks])
+    tokens = values = None
+    edge_dim = 0
+    if pairs is not None:
+        if len(pairs) != B:
+            raise ValueError(f'prefix_keys: edges must be a list of {B} per-cloud tensors')
+        floating = pairs[0].is_floating_point()
+        for c, t in enumerate(pairs):
+            want = torch.float32 if floating else torch.int64
+            if t.dtype != want or tuple(t.shape[:2]) != (seqlens[c], n_cur[c]) or t.dim() != (3 if floating else 2):
+                raise ValueError(f'prefix_keys: edges[{c}] must be {"float32 [m, n_cur, edge_dim]" if floating else "int64 [m, n_cur]"} '
+                                 f'with [m, n_cur] = {[seqlens[c], n_cur[c]]}, got {t.dtype} {tuple(t.shape)}')
+        flat = torch.cat([t.contiguous().reshape(-1) for t in pairs])
+        if floating:
+            values, edge_dim = flat, int(pairs[0].shape[2])
+        else:
+            tokens = flat
+    cu = [0]
+    for m in seqlens:
+        cu.append(cu[-1] + m)
+    dev = feats.device
+    desc = torch.tensor(cu + n_prev + off, dtype=torch.int64).to(dev)
+    feats, coors = feats.contiguous(), coors.contiguous()
+    out = torch.empty((M, 2), dtype=torch.int64, device=dev)
+    nbytes = 4 * feats.numel() + 12 * M + sum(t.numel() * t.element_size() for t in (tokens, values, nbr) if t is not None)
+    with torch.cuda.device(dev), _timed('prefix_keys', nbytes=nbytes):
+        _check(lib().se3_prefix_keys_fwd(_p(feats), M, feats.shape[1], _p(coors), _p(tokens), _p(values), edge_dim, _p(nbr),
+                                         _p(desc[:B + 1]), _p(desc[B + 1:2 * B + 1]),
+                                         _p(desc[2 * B + 1:]) if (pairs is not None or nbr is not None) else None, B, _p(out),
+                                         _stream()))
+    return out
 
 
 def gather_pairs(pair_feat, idx):
